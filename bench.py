@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- KVStore push+pull throughput on B200 (BASELINE.json metric).
+"""bench.py -- KVStore push+pull throughput on H100 (BASELINE.json metric).
 
 A *step* is one pass of the hot path over one batch of synthetic gradients: `pushpull` of the
 whole key set (sum over the ranks' gradients, fused SGD-momentum update of the stored fp32
@@ -13,7 +13,7 @@ weights, new weights delivered to every rank).  Workload (config.workload):
 One process per GPU (torchrun for N > 1); every rank contributes its own gradient for every key
 (weak scaling: per-GPU work is fixed).  `value` = N * 2 * S / t  [GB/s]: bytes pushed plus bytes
 pulled by all ranks per second, S = key-set bytes.  Inputs are larger than L2 (358 MB of
-gradients + 358 MB of weights + state per step vs 126 MB of L2), so no flush is needed.
+gradients + 358 MB of weights + state per step vs 50 MB of L2), so no flush is needed.
 
 Besides the contract's keys the line carries
   parity     the timed configuration (same arrays, same kernel variant) run once from a fresh store and compared
@@ -23,7 +23,12 @@ Besides the contract's keys the line carries
   secondary  BASELINE.json configs[2..4]: ResNet-50 / BERT-base bf16 training steps (samples/sec) through
              Trainer(kvstore='device'), row_sparse push + row_sparse_pull
 
+--dump-outputs DIR writes what the last timed step returned to the caller (the `out` arrays of pushpull) as
+DIR/out_<key>.npy, float32; keys are sampled at fixed seeded positions when the key set exceeds DUMP_ELEMS elements.
+Inputs are seeded, so two builds run with the same arguments can be compared output for output.
+
 Usage: python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload ...]
+                       [--dump-outputs DIR]
 """
 import argparse
 import json
@@ -153,8 +158,8 @@ def bind_to_gpu_numa(gpu_index):
 # ---------------------------------------------------------------------------
 # NVLink traffic as the hardware counts it (NVML field values, no profiler): DATA = payload bytes, RAW = payload +
 # protocol overhead, both directions, summed over the GPU's 18 links.  Read before and after the timed region,
-# the difference per step is the `traffic` of the N > 1 roofline (ncu cannot profile a kernel that rendezvous
-# with kernels on other GPUs: profiles/README.md).
+# the difference per step is the `traffic` of the N > 1 roofline (a kernel profiler cannot replay a kernel that
+# rendezvous with kernels on other GPUs).
 # ---------------------------------------------------------------------------
 _NVL_FIELDS = {"data_tx": 138, "data_rx": 139, "raw_tx": 140, "raw_rx": 141}     # NVML_FI_DEV_NVLINK_THROUGHPUT_*, KiB
 
@@ -188,10 +193,9 @@ class ClockSampler(object):
     """SM clock, max clock and throttle reasons of one GPU while the timed region runs.
 
     The samples come from NVML calls made by a thread of this process (clock info + current clocks-event reasons,
-    every 100 ms) -- NOT from an `nvidia-smi -lms` loop: on 8 GPUs that loop, at the 20 ms period round 2 first
-    used, slowed the NVSwitch-multicast exchange from 0.79 to 1.21 ms per step (profiles/r02_diag_n8_sampler.txt;
-    one GPU's queries stall all eight through the rendezvous), while at N = 1 / 2 it cost nothing.  Only when
-    pynvml is missing does the sampler fall back to `nvidia-smi -lms 250`."""
+    every 100 ms) -- NOT from an `nvidia-smi -lms` loop: on 8 GPUs a fast loop slows the NVSwitch-multicast
+    exchange (one GPU's queries stall all eight through the rendezvous).  Only when pynvml is missing does the
+    sampler fall back to `nvidia-smi -lms 250`."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -338,26 +342,6 @@ def cpu_kvstore_step_factory(shapes, n_values, threads, optimizer):
                                           weights[k].ctypes.data_as(O.c_f32p), ctypes.c_int64(e),
                                           ctypes.c_int(threads))
     return step
-
-
-def ncu_dram_bytes(path):
-    """dram__bytes_read.sum + dram__bytes_write.sum of the first kernel in an `ncu --page raw` text dump
-    (`metric  unit  value` or `metric  value  unit` columns)."""
-    units = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9, "Tbyte": 1e12}
-    got = {}
-    try:
-        with open(path) as f:
-            for line in f:
-                parts = line.split()
-                if len(parts) >= 3 and parts[0] in ("dram__bytes_read.sum", "dram__bytes_write.sum") \
-                        and parts[0] not in got:
-                    unit = [x for x in parts[1:] if x in units]
-                    num = [x for x in parts[1:] if x.replace(",", "").replace(".", "", 1).isdigit()]
-                    if unit and num:
-                        got[parts[0]] = float(num[-1].replace(",", "")) * units[unit[0]]
-    except OSError:
-        return None
-    return sum(got.values()) if len(got) == 2 else None
 
 
 def host_cpus():
@@ -761,7 +745,7 @@ def train_steps(env, args, which):
         torch._foreach_zero_(gl)
         return loss
 
-    steps, warm = min(args.steps, 30), max(3, args.warmup)
+    steps, warm = args.steps, max(3, args.warmup)
     for _ in range(warm):
         step()
     torch.cuda.synchronize(); env.barrier()
@@ -838,7 +822,7 @@ def bench_rsp(env, args):
         kv.push("emb", grad)
         kv.row_sparse_pull("emb", out=out, row_ids=ids)
 
-    steps, warm = min(max(args.steps, 20), 100), max(3, args.warmup)
+    steps, warm = args.steps, max(3, args.warmup)
     for _ in range(warm):
         step()
     torch.cuda.synchronize(); env.barrier()
@@ -859,7 +843,7 @@ def bench_rsp(env, args):
     # algorithmic bytes per GPU per step: read every rank's nnz rows (+ ids), read-modify-write weight and momentum
     # rows of the union (2 reads + 2 writes), then gather nnz rows out (read + write)
     alg = world * nnz * (row_bytes + 8) + int(all_idx.size) * row_bytes * 4 + nnz * row_bytes * 2
-    peak = measured_peaks().get("hbm_gbs", 6650.0)
+    peak = HBM_PEAK_GBS
     res = {"metric": "row_sparse push + row_sparse_pull rows/s", "value": world * nnz / (ms * 1e-3),
            "unit": "rows/s", "n_gpus": world, "steps": steps, "warmup": warm, "ms_per_step": ms,
            "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
@@ -875,18 +859,36 @@ def bench_rsp(env, args):
     return res
 
 
-_PEAKS = None
+# H100 SXM data sheet (700 W part): 3.35 TB/s of HBM3, 900 GB/s of NVLink (both directions together).  Data-sheet
+# peaks, not measured ones: the roofline fractions below are taken against them.
+HBM_PEAK_GBS = 3350.0
+NVLINK_PEAK_GBS_PER_DIR = 450.0
+
+# --dump-outputs: at most this many float32 elements (32 MB) in all
+DUMP_ELEMS = 8 << 20
 
 
-def measured_peaks():
-    global _PEAKS
-    if _PEAKS is None:
-        try:
-            with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-                _PEAKS = json.load(f)
-        except Exception:
-            _PEAKS = {}
-    return _PEAKS
+def dump_positions(shapes, budget=DUMP_ELEMS):
+    """Per key: None (dump the whole array) or the sorted flat positions of a fixed, seeded sample.  Keys are cut
+    to a common cap chosen so that the dump holds at most `budget` elements; a key below the cap is dumped whole."""
+    sizes = [nelem(s) for s in shapes]
+    if sum(sizes) <= budget:
+        return [None] * len(sizes)
+    lo, hi = 1, max(sizes)
+    while lo < hi:
+        mid = (lo + hi + 1) // 2
+        if sum(min(e, mid) for e in sizes) <= budget:
+            lo = mid
+        else:
+            hi = mid - 1
+    return [None if e <= lo else np.unique(np.random.default_rng(k).integers(0, e, lo)) for k, e in enumerate(sizes)]
+
+
+def dump_outputs(dirname, shapes, outs):
+    os.makedirs(dirname, exist_ok=True)
+    for k, (pos, o) in enumerate(zip(dump_positions(shapes), outs)):
+        a = o.asnumpy().reshape(-1)
+        np.save(os.path.join(dirname, "out_%03d.npy" % k), np.ascontiguousarray(a if pos is None else a[pos], np.float32))
 
 
 # ---------------------------------------------------------------------------
@@ -911,10 +913,16 @@ def main():
     ap.add_argument("--no-parity", action="store_true")
     ap.add_argument("--no-clocks", action="store_true", help="do not run the nvidia-smi clock sampler (diagnosis)")
     ap.add_argument("--no-nvml", action="store_true", help="do not read the NVML NVLink counters (diagnosis)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's pushpull outputs to DIR/out_<key>.npy")
     ap.add_argument("--local-world", type=int, default=0,
                     help="split the box into 'nodes' of this many GPUs and use kv.create('dist_device_sync'): NVLink "
                          "peer memory inside a node, NCCL between nodes (not the driver's configuration)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and args.workload in ("resnet50-train", "bert-train", "rsp"):
+        ap.error("--dump-outputs covers the pushpull workloads (sweep, resnet50, bert)")
     if args.optimizer is None:
         args.optimizer = "adam" if args.workload == "bert" else "sgd"
     rank = int(os.environ.get("RANK", 0))
@@ -940,7 +948,7 @@ def main():
         args.workload, len(shapes), S / 1e6, args.optimizer),
         "keys": len(shapes), "bytes_per_rank": S, "optimizer": args.optimizer,
         "parallelism": "dp%d (one process per GPU, gradient exchange over NVLink peer memory)" % args.gpus,
-        "l2": "working set (%.0f MB grads + weights + state per rank) exceeds the 126 MB L2; no flush" % (3 * S / 1e6)}
+        "l2": "working set (%.0f MB grads + weights + state per rank) exceeds the 50 MB L2; no flush" % (3 * S / 1e6)}
 
     if args.impl == "reference":
         if rank != 0:
@@ -1024,29 +1032,22 @@ def main():
     ms_total, kern_ms = env.max_over_ranks([ms_total, kern_ms])
     ms_step = ms_total / args.steps
     value = world * 2 * S / (ms_step * 1e-3) / 1e9
-    # clocks: the timed window is a few hundred ms at most -- every rank keeps the SAME steps running (untimed)
-    # until the GPU has been under this load for ~0.6 s, so that the 100 ms sampler sees it several times; the
-    # record covers both windows and says so
-    soak_steps = int(min(5000, max(0.0, 600.0 - ms_total) / max(ms_step, 1e-3)))
-    for _ in range(soak_steps):
-        step()
-    torch.cuda.synchronize(); env.barrier()
     t_host2 = time.time()
     clocks = None
     if rank == 0:
         clocks = sampler.stop(t_host0, t_host2)
-        clocks["window"] = "timed region (%d steps)%s" % (
-            args.steps, " + %d identical untimed steps (~0.6 s under load for the 100 ms sampler)" % soak_steps if soak_steps else "")
+        clocks["window"] = "timed region (%d steps)" % args.steps
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, shapes, weights)
 
     # ---- roofline for the dominant (only) kernel ------------------------------------------------
-    peaks = measured_peaks()
     nel = S // 4
     kname = "+".join(KERNEL_NAMES.get(v, v) for v in variant.split("+"))
     if world == 1:
         alg = nel * bytes_per_elem_n1
-        peak = peaks.get("hbm_gbs", 6650.0)
+        peak = HBM_PEAK_GBS
         roof = {"bound": "hbm", "achieved": alg / (kern_ms * 1e-3) / 1e9, "peak": peak, "unit": "GB/s",
-                "peak_source": "MEASURED_PEAKS.json hbm_gbs" if "hbm_gbs" in peaks else "fallback 6650",
+                "peak_source": "H100 SXM data sheet, 3.35 TB/s HBM3",
                 "traffic": None, "kernel": "kv_norm_first/(mid)/apply_kernel sequence" if layerwise else kname,
                 "kernel_ms": kern_ms, "algorithmic_bytes_per_launch": alg}
         if args.optimizer == "sgd":
@@ -1062,8 +1063,8 @@ def main():
         else:
             alg = 2.0 * S * (world - 1) / world      # per GPU per direction (tools/bandwidth/measure.py:138)
             kname += " (peer loads + fused update + peer stores)"
-        roof = {"bound": "nvlink", "achieved": alg / (kern_ms * 1e-3) / 1e9, "peak": 770.0, "unit": "GB/s",
-                "peak_source": "B200_PROFILING.md measured peer copy 770 GB/s/dir (900 nominal)",
+        roof = {"bound": "nvlink", "achieved": alg / (kern_ms * 1e-3) / 1e9, "peak": NVLINK_PEAK_GBS_PER_DIR,
+                "unit": "GB/s", "peak_source": "H100 SXM data sheet, NVLink 900 GB/s both directions together",
                 "traffic": None, "kernel": kname, "kernel_ms": kern_ms,
                 "algorithmic_bytes_per_launch": alg,
                 "note": "bytes that must cross this GPU's NVLink per direction; busbw_gbs_per_gpu is the "
@@ -1080,11 +1081,6 @@ def main():
             roof["nvlink_payload_efficiency"] = {"tx": per["data_tx"] / max(per["raw_tx"], 1.0), "rx": per["data_rx"] / max(per["raw_rx"], 1.0)}
         else:
             roof["traffic_error"] = (nvl0 or {}).get("error") or (nvl1 or {}).get("error")
-    # DRAM / NVLink bytes of the same kernel on the same workload from this round's ncu capture (bench.py
-    # cannot run under ncu itself: a number printed under a profiler is never a bench value)
-    tsrc = os.path.join(ROOT, "profiles", "r02_n%d_%s_ncu_full.txt" % (world, variant.replace("+", "_")))
-    if args.workload == "sweep" and args.optimizer == "sgd" and os.path.exists(tsrc):
-        roof["traffic"], roof["traffic_source"] = ncu_dram_bytes(tsrc), os.path.relpath(tsrc, ROOT)
 
     # ---- parity of what was just timed --------------------------------------------------------------
     parity, kept = {"checked": False}, None

@@ -1,5 +1,5 @@
 /*
- * mxkv_b200.h -- C ABI of the B200-native KVStore engine.
+ * mxkv_b200.h -- C ABI of the H100-native KVStore engine.
  *
  * Drop-in boundary: every MX* symbol below has the signature, argument meaning and
  * error behaviour (0 = ok, -1 = error, message via MXGetLastError(), never throws) of
@@ -140,7 +140,7 @@ MXKV_DLL int MXKVStoreRunServer(KVStoreHandle handle, MXKVStoreServerController 
                                 void* controller_handle);                                /* c_api.h:2797 */
 MXKV_DLL int MXKVStoreSendCommmandToServers(KVStoreHandle handle, int cmd_id, const char* cmd_body); /* :2808 */
 
-/* ---- B200 extensions ------------------------------------------------------ */
+/* ---- MXKVB200 extensions -------------------------------------------------- */
 /* Fused optimizer: what Python's Updater + sgd_update/adam_update ops do per key in the
  * reference (python/mxnet/optimizer/updater.py:39-93) happens inside the reduce kernel.
  * name: "sgd" | "adam" | "adamw" | "test" | "lamb" | "lans" | "lars"; kwargs use the reference's

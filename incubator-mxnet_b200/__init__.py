@@ -1,9 +1,9 @@
-"""B200-native KVStore engine behind MXNet's KVStore API.
+"""H100-native KVStore engine behind MXNet's KVStore API.
 
 Python host side: a ctypes binding of the C ABI in ``include/mxkv_b200.h`` shaped like the
 reference's ``python/mxnet/kvstore`` package (``create``, ``KVStoreBase`` registry, native
 ``KVStore`` wrapper) plus the minimal ``NDArray``/``Context``/``optimizer`` surface that
-package needs.  Everything numerical happens in ``libmxkv_b200.so`` (CUDA, sm_100a); there
+package needs.  Everything numerical happens in ``libmxkv_b200.so`` (CUDA, sm_90a); there
 is no CPU fallback -- calls fail with ``MXNetError`` when no GPU / no native library exists.
 """
 from . import base

@@ -1,7 +1,6 @@
-"""Build the in-tree native library ``incubator-mxnet_b200/libmxkv_b200.so`` for sm_100a.
+"""Build the in-tree native library ``incubator-mxnet_b200/libmxkv_b200.so`` for sm_90a (H100).
 
-nvcc cross-compiles without a GPU; the resulting .so travels to the GPU box with the
-repository snapshot (it is git-ignored, not gpurun-ignored).
+nvcc cross-compiles without a GPU; the library and its objects are build products (git-ignored).
 """
 import os
 import subprocess
@@ -12,7 +11,8 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libmxkv_b200.so")
 SOURCES = ["kernels.cu", "tree_kernels.cu", "rsp_kernels.cu", "norm_kernels.cu", "kvstore_norm.cc", "runtime.cc", "vmm_arena.cc", "topology.cc", "ndarray.cc", "kvstore.cc", "kvstore_rsp.cc", "c_api.cc"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
+FLAGS = GENCODE + ["-lineinfo", "-O3", "-std=c++17",
          "-Xcompiler", "-fPIC,-fvisibility=hidden,-Wall", "--threads", "4"]
 
 
@@ -52,7 +52,7 @@ def build(force=False, verbose=False):
             print(out.decode())
     if failed:
         raise RuntimeError("native build failed")
-    cmd = [NVCC, "-shared", "-o", OUT] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"]
+    cmd = [NVCC, "-shared", "-o", OUT] + objs + GENCODE
     subprocess.check_call(cmd)
     return OUT
 

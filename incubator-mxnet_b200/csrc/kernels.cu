@@ -1,4 +1,4 @@
-// kernels.cu -- sm_100a kernels of the KVStore gradient path.
+// kernels.cu -- sm_90a kernels of the KVStore gradient path.
 //
 // kv_dense_kernel: ONE kernel does what the reference spreads over
 //   n x CopyFromTo (cudaMemcpyPeerAsync, src/ndarray/ndarray_function.cu:68-99)
@@ -263,12 +263,12 @@ kv_dense_bulk_kernel(DenseLaunch L) {
   if (sync) barrier_start(L.sync);     // no peer byte may be requested before the rendezvous
 
   // tiles of this block: groups of G consecutive tiles, block-cyclic -- tile(i) = ((i / G) * grid + block) * G + i % G.
-  // G = 1 is the plain strided walk: all blocks stream through one narrow window of every array (best for DRAM:
-  // 0.945 of the measured HBM peak on the 256 MB sweep keys) but every block meets every key of the work list and
-  // reloads a 400-byte descriptor each time, which cost a fifth of the kernel on a 199-key model (BERT-base:
-  // 0.78).  A contiguous range per block has the opposite profile (0.83 / 0.90).  Small groups keep the window
-  // narrow and divide the descriptor switches by G (profiles/r02_tune_bulk_group.txt); the host groups only work
-  // lists of many keys (kvstore.cc: LaunchWorks) and keeps G = 1 for the rest.
+  // G = 1 is the plain strided walk: all blocks stream through one narrow window of every array (best for DRAM on
+  // large keys) but every block meets every key of the work list and reloads a 400-byte descriptor each time, which
+  // costs a large share of the kernel on a model of hundreds of small keys (BERT-base).  A contiguous range per
+  // block has the opposite profile.  Small groups keep the window narrow and divide the descriptor switches by G
+  // (MXKV_B200_BULK_GROUP); the host groups only work lists of many keys (kvstore.cc: LaunchWorks) and keeps G = 1
+  // for the rest.
   const int64_t G = L.bulk_group > 0 ? L.bulk_group : 1;
   int64_t ntiles;
   if (G == 1) {             // the plain strided walk, without the divisions of the grouped one
@@ -456,7 +456,7 @@ __device__ __forceinline__ void mm_st(void* p, const float4& v) {
 //         all-gather half (the two halves use opposite link directions)
 // The SM side is never the limiter here (a GPU consumes ~80 GB/s of reduced data, i.e. < 1 KB/us per SM): what
 // these knobs and the grid size change is the REQUEST PATTERN the switch sees (how many reduce requests queue
-// in the fabric, how they interleave with the multicast stores).  Measured choices: profiles/r02_nvls_tune.txt.
+// in the fabric, how they interleave with the multicast stores).  tools/tune_nvls.py sweeps them.
 struct NvlsChunk {
   const float* g;      // multicast address of the key's gradient
   int64_t cb, ce;      // element range of the chunk
@@ -720,10 +720,10 @@ static DenseKernelFn pick_kernel(const DenseLaunch& L) {
 static int g_num_sms[64] = {0};
 
 static int sm_count(int device) {
-  if (device < 0 || device >= 64) return 148;
+  if (device < 0 || device >= 64) return kNumSms;
   if (g_num_sms[device] == 0) {
     int n = 0;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || n <= 0) n = kNumSms;
     g_num_sms[device] = n;
   }
   return g_num_sms[device];
@@ -765,9 +765,9 @@ int BulkPlan(int device, int opt, int multi_precision, int arrays, int* tile_ele
     if (g_smem_budget < 16 * 1024) g_smem_budget = 16 * 1024;
     if (g_smem_budget > 200 * 1024) g_smem_budget = 200 * 1024;
   }
-  // measured on B200 (profiles/r01_tune_bulk.txt): 2048-element tiles, two stages; deeper rings or
-  // smaller tiles are slower.  Wide work lists (many sources) fall back to 1024-element tiles to keep
-  // two blocks per SM resident.
+  // 2048-element tiles, two stages (MXKV_B200_BULK_TILE / _STAGES override them): with two blocks per SM
+  // that is 2 x 100 KB of the 228 KB of shared memory an H100 SM has.  Wide work lists (many sources) fall
+  // back to 1024-element tiles to keep two blocks per SM resident.
   int tile = 2048;
   int st = 2;
   if (st * arrays * tile * 4 > g_smem_budget) tile = 1024;
@@ -849,7 +849,7 @@ int LaunchCastToF32(const void* src, int dtype, float* dst, int64_t n, cudaStrea
   if (n == 0) return 0;
   const int threads = 256;
   int64_t blocks = (n + threads - 1) / threads;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > kMaxBlocks) blocks = kMaxBlocks;
   switch (dtype) {
     case kFloat32: kv_cast_f32_kernel<float><<<blocks, threads, 0, s>>>(static_cast<const float*>(src), dst, n); break;
     case kFloat16: kv_cast_f32_kernel<__half><<<blocks, threads, 0, s>>>(static_cast<const __half*>(src), dst, n); break;
@@ -887,7 +887,7 @@ int LaunchQuantize(int bits, const float* grad, float* residual, uint32_t* out, 
   if (n == 0) return 0;
   const int per = 32 / bits;
   int64_t blocks = ((n + per - 1) / per + 255) / 256;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > kMaxBlocks) blocks = kMaxBlocks;
   if (blocks < 1) blocks = 1;
   if (bits == 2) kv_quantize_kernel<2><<<blocks, 256, 0, s>>>(grad, residual, out, n, thr);
   else if (bits == 1) kv_quantize_kernel<1><<<blocks, 256, 0, s>>>(grad, residual, out, n, thr);
@@ -898,7 +898,7 @@ int LaunchQuantize(int bits, const float* grad, float* residual, uint32_t* out, 
 int LaunchDequantize(int bits, const uint32_t* in, float* out, int64_t n, float thr, cudaStream_t s) {
   if (n == 0) return 0;
   int64_t blocks = (n + 255) / 256;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > kMaxBlocks) blocks = kMaxBlocks;
   if (bits == 2) kv_dequantize_kernel<2><<<blocks, 256, 0, s>>>(in, out, n, thr);
   else if (bits == 1) kv_dequantize_kernel<1><<<blocks, 256, 0, s>>>(in, out, n, thr);
   else return static_cast<int>(cudaErrorInvalidValue);

@@ -1,5 +1,5 @@
 // kernels.h -- device work descriptors and launcher entry points shared between
-// the host runtime (engine.cc) and the sm_100a kernels (kernels.cu).
+// the host runtime (engine.cc) and the sm_90a kernels (kernels.cu).
 //
 // One launch of the dense kernel processes a *work list*: every entry is one key
 // (or the shard of a key this rank owns) with up to kMaxSrc gradient sources and
@@ -15,7 +15,8 @@ namespace mxkv {
 constexpr int kMaxSrc = 16;      // values per key in one push (reference tests use 4; 8 GPUs => 8)
 constexpr int kMaxOut = 24;      // n store replicas + n user outputs + merge buffers
 constexpr int kMaxRanks = 8;     // one NVSwitch domain
-constexpr int kMaxBlocks = 1184; // 148 SMs x 8
+constexpr int kNumSms = 132;     // H100 SXM; launches query the device, this is the fallback
+constexpr int kMaxBlocks = kNumSms * 8;
 constexpr int kChunkElems = 8192;   // default elements per scheduling chunk (MXKV_B200_CHUNK)
 
 // mshadow type flags, 3rdparty/mshadow/mshadow/base.h:352-366

@@ -569,7 +569,7 @@ int KVStore::DefaultDevice() {
   Runtime* rt = Runtime::Get();
   if (rt->pg()) return rt->pg()->dev();
   MXKV_CHECK(rt->NumDevices() > 0)
-      << "no CUDA device is visible: the B200 KVStore has no CPU fallback (build/run it on a GPU box)";
+      << "no CUDA device is visible: this KVStore has no CPU fallback (build/run it on a GPU box)";
   return 0;
 }
 
@@ -1899,8 +1899,8 @@ void KVStore::ReduceUpdate(std::vector<Group>& groups, bool write_outs) {
       // NVLS: every array of the key is bound to a multicast object (and nothing has to be copied
       // out of a complete replica afterwards)
       // (auto: above 4 ranks.  Per direction the switch path moves S(1 + 1/n) against 2S(n-1)/n of
-      // the peer path: 1.5x more at n=2, equal time measured at n=4 -- where the peer path is kept
-      // because it is bit-exact --, 1.56x less at n=8: busbw 782 vs 641 GB/s, profiles/r01_tune_bulk.txt)
+      // the peer path: 1.5x more at n=2, 1.2x less at n=4 -- where the peer path is still kept because
+      // it is bit-exact --, 1.56x less at n=8)
       if (mp_mode && collective && !hier_ && tree_plan == nullptr &&
           (rt->nvls_mode >= 2 || (rt->nvls_mode == 1 && n_part > 4)) &&
           !(fused && IsNormOpt(opt_.kind)) && ks.dtype == kFloat32 && ks.size % 4 == 0 &&
@@ -2159,12 +2159,11 @@ void KVStore::LaunchWorks(const LaunchClassKey& ck, std::vector<std::vector<Tens
     const int extra = (opt_kind != OPT_NONE ? 1 : 0) +
                       ((opt_kind == OPT_SGD_MOM || opt_kind == OPT_ADAM || opt_kind == OPT_ADAMW) ? 1 : 0) +
                       ((opt_kind == OPT_ADAM || opt_kind == OPT_ADAMW) ? 1 : 0);
-    // measured (profiles/r01_tune_bulk.txt): the staged variant wins (a) whenever sources are read
-    // over NVLink (busbw 623 vs 575 GB/s at n=2, 664 vs 637 at n=4: more bytes in flight against a
-    // ~2 us round trip) and (b) locally when a thread of the per-thread variant would have few loads
-    // in flight (<= 2 sources, >= 3 streams: 6255 vs 5413 GB/s at n=1).  With >= 3 local sources the
-    // per-thread variant already keeps enough requests in flight and is faster (6606 vs 5794 GB/s at
-    // n=4 on one GPU).  bulk_mode 2 forces the staged variant wherever it is eligible.
+    // the staged variant is taken (a) whenever sources are read over NVLink (more bytes in flight
+    // against a ~2 us round trip) and (b) locally when a thread of the per-thread variant would have
+    // few loads in flight (<= 2 sources, >= 3 streams).  With >= 3 local sources the per-thread variant
+    // already keeps enough requests in flight.  bulk_mode 2 forces the staged variant wherever it is
+    // eligible.
     const bool want = rt->bulk_mode >= 2 || ck.sync_mode != SYNC_NONE || (max_src <= 2 && max_src + extra >= 3);
     if (ok && want) {
       // n_src is the same for every entry of a collective class; take the max for safety

@@ -1,5 +1,5 @@
 // kvstore.h -- KVStoreLocal semantics (src/kvstore/kvstore_local.h:70-552) on top of
-// the fused sm_100a reduce/update/broadcast kernel.
+// the fused sm_90a reduce/update/broadcast kernel.
 //
 // What is kept from the reference: the API and its observable behaviour -- key
 // bookkeeping (int or str keys, never mixed, :344-347), duplicate-init check (:230-233),
@@ -152,7 +152,7 @@ class KVStore {
   void SetGradientCompression(const std::vector<std::pair<std::string, std::string>>& kwargs);
   void Barrier();
 
-  // fused optimizer (B200 extension; replaces the Python Updater round trip)
+  // fused optimizer (MXKVB200 extension; replaces the Python Updater round trip)
   void SetOptimizer(const std::string& name, const std::vector<std::pair<std::string, std::string>>& kwargs);
   void SetOptimizerMult(bool str_key, int ikey, const std::string& skey, float lr_mult, float wd_mult);
   // type 'updater' only: in-place fused update of caller-owned (weight, grad) pairs (kvstore.cc)

@@ -1,4 +1,4 @@
-// kvstore_rsp.cc -- row_sparse push / row_sparse_pull of KVStoreLocal on the B200 kernels.
+// kvstore_rsp.cc -- row_sparse push / row_sparse_pull of KVStoreLocal on the H100 kernels.
 //
 // Reference: CommDevice::ReduceRowSparse (src/kvstore/comm.h:479-502) copies every row_sparse
 // source to one GPU and calls the row_sparse ElementwiseSum; the updater then runs a sparse

@@ -1,4 +1,4 @@
-// norm_kernels.cu -- sm_100a kernels of the layer-wise adaptive optimizers (see norm_kernels.h).
+// norm_kernels.cu -- sm_90a kernels of the layer-wise adaptive optimizers (see norm_kernels.h).
 //
 // Element arithmetic follows the reference's CPU kernels operation by operation
 // (contrib/multi_lamb.cc:36-120, contrib/multi_lans.cc:36-130, optimizer_op-inl.h:377-390,590-606
@@ -421,7 +421,7 @@ int NormMaxGrid(int device) {
   static int cache[64] = {0};
   if (device >= 0 && device < 64 && cache[device] > 0) return cache[device];
   int sms = 0;
-  if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || sms <= 0) sms = 148;
+  if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || sms <= 0) sms = kNumSms;
   int occ = 2, o = 0;
   if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o, kv_norm_first_kernel<__half, true, false>, kNormThreads, 0) ==
           cudaSuccess && o > 0) occ = o < occ ? o : occ;

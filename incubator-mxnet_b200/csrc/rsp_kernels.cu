@@ -479,7 +479,7 @@ __global__ void rsp_set_i64_kernel(int64_t* p, int64_t v) { *p = v; }
 static int grid_for(int64_t items, int per_block) {
   int64_t g = (items + per_block - 1) / per_block;
   if (g < 1) g = 1;
-  if (g > 148 * 8) g = 148 * 8;
+  if (g > kMaxBlocks) g = kMaxBlocks;
   return static_cast<int>(g);
 }
 
@@ -538,9 +538,9 @@ int LaunchRspPushFused(int device, const RspSources& S, const RspRowArgs& A, con
   if (c == 0) c = resident_grid(device, reinterpret_cast<const void*>(fn), 256, 0);
   if (c < 1) return static_cast<int>(cudaErrorLaunchOutOfResources);
   int64_t want = (est_rows + 7) / 8;
-  if (St.publish) want = std::max<int64_t>(want, 148);      // the staging copy wants the whole machine
+  if (St.publish) want = std::max<int64_t>(want, kNumSms);      // the staging copy wants the whole machine
   // two blocks per SM are plenty for a gather, and every block more makes the in-kernel barriers dearer
-  const int grid = static_cast<int>(std::max<int64_t>(1, std::min<int64_t>(std::min<int64_t>(c, 296), want)));
+  const int grid = static_cast<int>(std::max<int64_t>(1, std::min<int64_t>(std::min<int64_t>(c, 2 * kNumSms), want)));
   fn<<<grid, 256, 0, stream>>>(S, A, St, sync);
   return static_cast<int>(cudaGetLastError());
 }
@@ -626,7 +626,7 @@ __global__ void rsp_cast_ids_kernel(const T* src, int64_t* dst, int64_t n) {
 int LaunchCastIdsToI64(const void* src, int dtype, int64_t* dst, int64_t n, cudaStream_t stream) {
   if (n <= 0) return 0;
   const int threads = 256;
-  const int grid = static_cast<int>(std::min<int64_t>((n + threads - 1) / threads, 1184));
+  const int grid = static_cast<int>(std::min<int64_t>((n + threads - 1) / threads, kMaxBlocks));
   switch (dtype) {
     case kFloat32: rsp_cast_ids_kernel<float><<<grid, threads, 0, stream>>>(static_cast<const float*>(src), dst, n); break;
     case kFloat64: rsp_cast_ids_kernel<double><<<grid, threads, 0, stream>>>(static_cast<const double*>(src), dst, n); break;

@@ -55,7 +55,7 @@ struct DeviceState {
   cudaEvent_t ev_xdev = nullptr;
   uint32_t* signal_pad = nullptr;      // this device's pad (SP mode: cudaMalloc; MP mode: in the arena)
   StagingRing ring;
-  int max_grid = 296;
+  int max_grid = 2 * kNumSms;
   bool engine_dirty = false;           // engine stream has work the user stream has not been fenced on
   // host-resident values: H2D / compute / D2H software pipeline (kvstore.cc: HostPipelined)
   static constexpr int kHostSlots = 3;
@@ -168,9 +168,8 @@ class Runtime {
   int nvls_unroll = 2;                       // MXKV_B200_NVLS_U: ld_reduce requests in flight per thread (1 | 2 | 4 | 8)
   int nvls_pipe = 0;                         // MXKV_B200_NVLS_PIPE: issue the next chunk's ld_reduce before this chunk's update
   int nvls_grid = 48;                        // MXKV_B200_NVLS_GRID: cap on the multicast kernel's grid (0: resident capacity).
-                                             // The switch, not the SMs, bounds this kernel: 24-64 blocks are 3-4 % faster than
-                                             // a full grid at 8 ranks and leave 100 SMs to whatever else is running
-                                             // (profiles/r02_nvls_tune_n8.txt)
+                                             // The switch, not the SMs, bounds this kernel: a small grid leaves most
+                                             // SMs to whatever else is running (tools/tune_nvls.py sweeps it)
   int nvls_threads = 512;                    // MXKV_B200_NVLS_THREADS: its block size (128 | 256 | 512)
   int bulk_mode = 1;                         // MXKV_B200_BULK: 0 off, 1 auto (<= 2 sources), 2 whenever eligible
   int bulk_group = 4;                        // MXKV_B200_BULK_GROUP: consecutive tiles per block of the staged kernel,

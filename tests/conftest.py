@@ -27,7 +27,7 @@ def pytest_runtest_call(item):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA GPU (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA GPU (an H100)")
     config.addinivalue_line("markers", "multigpu: needs >= 2 GPUs")
 
 

@@ -1,4 +1,4 @@
-"""Regenerates tests/golden/*.npz.  Runs ONLY in the authoring container (needs /root/reference):
+"""Regenerates tests/golden/*.npz and *.json.  Needs the reference source tree (REF) and oracle/_ref built from it:
 
 * dense_sums.npz   -- outputs of the reference's own mshadow arithmetic (oracle/_ref/libkvref.so,
                       built from /root/reference/3rdparty/mshadow by oracle/Makefile) for the
@@ -24,8 +24,20 @@
                       mesh of its comments, random matrices of 2 ... 16 GPUs with and without missing links --
                       by Kernighan-Lin and by the exhaustive search; plus the outcome of one Kernighan-Lin pass.
 
-The GPU box has no /root/reference; tests read the committed fixtures instead.
+* dense_sums_live.npz -- the reference's mshadow sums (oracle/_ref/libkvref.so) of the seeded inputs
+                      test_oracle_golden.py::test_dense_sum_against_live_reference_arithmetic draws: per case the
+                      first 64 values and a SHA-256 of all output bytes.
+
+* tree_topology_draw.npz -- the trees the reference's compiled header builds for the fixed draw of random link
+                      matrices of test_topology.py::test_trees_match_the_reference_header_compiled_in_place.
+
+* c_api_prototypes.json -- parameter types of every function include/mxkv_b200.h shares with the reference's
+                      include/mxnet/c_api.h, parsed from the reference header (test_abi.py::c_prototypes).
+
+The tests read the committed fixtures; none of them needs the reference tree.
 """
+import hashlib
+import json
 import ast
 import os
 import sys
@@ -449,6 +461,67 @@ def tree_topology():
     print("tree_topology: %d matrices (%d without a tree), %d Kernighan-Lin passes" % (len(cases), fails, len(kl)))
 
 
+def bits_digest(a):
+    """SHA-256 of an array's bytes (C order): the golden form of an output too large to store whole."""
+    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
+
+
+def dense_sums_live():
+    """The inputs test_dense_sum_against_live_reference_arithmetic draws, summed by the reference's arithmetic."""
+    from oracle import oracle as O
+    assert O.ref_lib() is not None, "build oracle/_ref first (make -C oracle)"
+    out = {}
+    rng = np.random.default_rng(5)
+    for n in (2, 3, 4, 5, 6, 8, 9, 13):
+        for E in (1, 17, 5000):
+            vals = [rng.uniform(-1, 1, E).astype(np.float32) for _ in range(n)]
+            d = [v.astype(np.float64) for v in vals]
+            i = [(v * 1000).astype(np.int32) for v in vals]
+            for kind, r in (("device_f32", O.ref_sum_device(vals)), ("commcpu_f32", O.ref_sum_cpu(vals)),
+                            ("device_f64", O.ref_sum_device(d)), ("device_i32", O.ref_sum_device(i))):
+                tag = "%s_n%d_E%d" % (kind, n, E)
+                out[tag + "_head"] = r[:64]
+                out[tag + "_sha256"] = np.array(bits_digest(r))
+    np.savez_compressed(os.path.join(HERE, "dense_sums_live.npz"), **out)
+
+
+def tree_topology_draw():
+    """The fixed draw of test_trees_match_the_reference_header_compiled_in_place and the reference's trees for it."""
+    from oracle import oracle as O
+    assert O.ref_topology_lib() is not None, "build oracle/_ref first (make -C oracle)"
+    rng = np.random.default_rng(20260921)
+    out, i = {}, 0
+    for n in (2, 3, 4, 5, 6, 7, 8, 9, 11, 13, 16):
+        for rep in range(3):
+            u = rng.uniform(0, 1, (n, n))
+            W = np.where(u < 0.33, 1.0, np.where(u < 0.66, 2.0, 3.0))
+            if rep % 3 == 2:
+                W = np.where(rng.uniform(0, 1, (n, n)) < 0.3, 0.0, W)
+            W = np.triu(W, 1)
+            W = (W + W.T).astype(np.float32)
+            alpha = float(rng.choice([0.7, 0.5, 0.9]))
+            for bt in ((False, True) if n <= 5 else (False,)):
+                out["case_%d_W" % i], out["case_%d_alpha" % i], out["case_%d_backtrack" % i] = W, np.float32(alpha), np.array(bt)
+                want = O.ref_compute_trees(W, alpha, bt)
+                if want is None:
+                    out["case_%d_fails" % i] = np.array(1)
+                else:
+                    out["case_%d_topo" % i], out["case_%d_scan" % i] = want[0].astype(np.int16), want[1].astype(np.int16)
+                i += 1
+    out["n_cases"] = np.array(i)
+    np.savez_compressed(os.path.join(HERE, "tree_topology_draw.npz"), **out)
+
+
+def c_api_prototypes():
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    from test_abi import c_prototypes
+    ref = c_prototypes(os.path.join(REF, "include", "mxnet", "c_api.h"), "MXNET_DLL")
+    mine = c_prototypes(os.path.join(ROOT, "include", "mxkv_b200.h"), "MXKV_DLL")
+    with open(os.path.join(HERE, "c_api_prototypes.json"), "w") as f:
+        json.dump({n: ref[n] for n in sorted(mine) if n in ref}, f, indent=0, sort_keys=True)
+        f.write("\n")
+
+
 if __name__ == "__main__":
     if len(sys.argv) > 1:                 # e.g. `make_golden.py tree_topology`: only the named fixtures
         for name in sys.argv[1:]:
@@ -461,4 +534,7 @@ if __name__ == "__main__":
     sparse_steps()
     lr_schedules()
     tree_topology()
-    print("wrote", sorted(f for f in os.listdir(HERE) if f.endswith(".npz")))
+    dense_sums_live()
+    tree_topology_draw()
+    c_api_prototypes()
+    print("wrote", sorted(f for f in os.listdir(HERE) if f.endswith((".npz", ".json"))))

@@ -1,6 +1,7 @@
 """Worker of tests/test_gpu_multi.py::test_mp_one_process_per_gpu (launched by torchrun).
 Every rank regenerates every rank's data from seeds, so each can check itself against the oracle."""
 import os
+import shutil
 import sys
 import tempfile
 
@@ -212,13 +213,15 @@ def main():
                 assert bits_equal(outs[k].asnumpy(), want), (optname, step, k)
         if optname == "adam":
             # sharded state: save on every rank (gathers), reload into a fresh store, continue
-            f = os.path.join(tempfile.gettempdir(), "mxkv_states_%d_%d" % (world, rank))
+            # a private directory: a fixed name under /tmp may be held by another user's earlier run
+            f = os.path.join(tempfile.mkdtemp(prefix="mxkv_states_"), "states_%d_%d" % (world, rank))
             kv2.save_optimizer_states(f, dump_optimizer=True)     # with its update counts
             mids = [o.asnumpy() for o in outs]
             kv3 = mx.kv.create("device")
             kv3.init(ks, [mx.nd.array(m, ctx) for m in mids])
             kv3.set_optimizer(mx.optimizer.create(optname, **kw))
             kv3.load_optimizer_states(f)
+            shutil.rmtree(os.path.dirname(f))
             outs3 = [mx.nd.empty(s, ctx) for s in shapes]
             for k, s in zip(ks, shapes):
                 gsym[k][:] = data(900 + k, s, rank)

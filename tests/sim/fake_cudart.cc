@@ -154,8 +154,8 @@ API cudaError_t cudaDeviceGetP2PAttribute(int* value, cudaDeviceP2PAttr, int, in
 API cudaError_t cudaDeviceGetStreamPriorityRange(int* lo, int* hi) { *lo = 0; *hi = -5; return cudaSuccess; }
 API cudaError_t cudaDeviceGetAttribute(int* v, cudaDeviceAttr attr, int) {
   switch (attr) {
-    case cudaDevAttrMultiProcessorCount: *v = 148; break;
-    case cudaDevAttrClockRate: *v = 1965000; break;
+    case cudaDevAttrMultiProcessorCount: *v = 132; break;
+    case cudaDevAttrClockRate: *v = 1980000; break;
     case cudaDevAttrMaxSharedMemoryPerBlockOptin: *v = 227 * 1024; break;
     default: *v = 0; break;
   }

@@ -1,5 +1,4 @@
-"""Semantics added late in round 1 and, unlike the files that sort before this one, not yet run on a B200 when they were
-committed (DESIGN.md §10 item 0): update counts that follow the Python optimizer, a new optimizer starting from fresh
+"""Semantics added late in round 1 (DESIGN.md §10 item 0): update counts that follow the Python optimizer, a new optimizer starting from fresh
 state, row_sparse gradients for dense keys, user-defined Python optimizers on the store, the reference's
 `test_sparse_aggregator` / bandwidth-tool / many-array `multi_sum_sq` cases.  They pass on the simulated runtime
 (tests/sim); the file name keeps them behind the hardware-validated tests in a `pytest -x` run."""

@@ -268,6 +268,14 @@ def test_bench_helpers_without_a_gpu():
     assert all(np.array_equal(x, y) for x, y in zip(a, b)) and not np.array_equal(a[1], bench.rank_grads(4, small)[1])
     big = a[1]                                         # above 2^20 elements: a random block of 1 000 003 elements, repeated
     assert np.array_equal(big[:1000003][:1000], big[1000003:1000003 + 1000]) and big.dtype == np.float32
+    # --dump-outputs: the same positions every run, within the budget; small key sets are dumped whole
+    for wl in ("sweep", "resnet50", "bert"):
+        shapes = bench.keyset(wl)
+        pos, again = bench.dump_positions(shapes), bench.dump_positions(shapes)
+        assert sum(bench.nelem(s) if p is None else p.size for s, p in zip(shapes, pos)) <= bench.DUMP_ELEMS
+        assert all((p is None and q is None) or np.array_equal(p, q) for p, q in zip(pos, again))
+        assert all(p is None or (np.all(np.diff(p) > 0) and p[-1] < bench.nelem(s)) for s, p in zip(shapes, pos))
+    assert bench.dump_positions(small) == [None, None]
     # clock sampler on a stand-in pynvml
     fake = types.ModuleType("pynvml")
     fake.NVML_CLOCK_SM = 1

@@ -4,8 +4,8 @@
 Three pins, strongest first:
 * tests/golden/tree_topology.npz: trees the reference's compiled header produced for 136 link matrices (one
   switch, the NVLink cube mesh, random 2 ... 16 GPUs; Kernighan-Lin and exhaustive search) -- always checked;
-* oracle/_ref/libkvref_topo.so, the reference header compiled in place: random matrices (a fixed draw; fresh ones in soak runs), when the
-  library is there (authoring container; it travels to the GPU box prebuilt);
+* the reference header compiled in place (oracle/_ref/libkvref_topo.so) on random matrices: a fixed draw whose trees
+  are stored in tests/golden/tree_topology_draw.npz, and fresh draws in soak runs where that library is built;
 * the known answers of the reference's unit test, tests/cpp/kvstore/gpu_topology_test.cc, function by function.
 Then the derived add schedules: the kernel's own evaluator (csrc/tree_math.h compiled for the host) against the
 oracle's level-by-level restatement of CommDeviceTree::ReduceInner on every golden tree."""
@@ -54,28 +54,38 @@ def test_kernighan_lin_pass_matches_the_reference_golden(golden):
         assert [int(v) for p in pairs for v in p] == golden["kl_%d_pairs" % i].tolist()
 
 
-@pytest.mark.skipif(O.ref_topology_lib() is None, reason="oracle/_ref/libkvref_topo.so not built (no /root/reference)")
 def test_trees_match_the_reference_header_compiled_in_place():
-    # a fixed draw in the gating suite; MXKV_FUZZ_SEEDS > 0 (soak runs): fresh matrices every time
-    fresh = int(os.environ.get("MXKV_FUZZ_SEEDS", "0")) > 0
-    rng = np.random.default_rng(int.from_bytes(os.urandom(4), "little") if fresh else 20260921)
-    for n in (2, 3, 4, 5, 6, 7, 8, 9, 11, 13, 16):
-        for rep in range(3):
-            u = rng.uniform(0, 1, (n, n))
-            W = np.where(u < 0.33, 1.0, np.where(u < 0.66, 2.0, 3.0))
-            if rep % 3 == 2:
-                W = np.where(rng.uniform(0, 1, (n, n)) < 0.3, 0.0, W)
-            W = np.triu(W, 1)
-            W = (W + W.T).astype(np.float32)
-            alpha = float(rng.choice([0.7, 0.5, 0.9]))
-            for bt in ((False, True) if n <= 5 else (False,)):
-                want = O.ref_compute_trees(W, alpha, bt)
-                if want is None:
-                    with pytest.raises(mx.MXNetError):
-                        T.compute_trees(W, alpha, bt)
-                    continue
-                topo, scan, _ = T.compute_trees(W, alpha, bt)
-                assert np.array_equal(topo, want[0]) and np.array_equal(scan, want[1]), (n, rep, bt, W.tolist())
+    # the fixed draw against the stored trees; MXKV_FUZZ_SEEDS > 0 (soak runs): fresh matrices every time, against
+    # the reference header compiled in place
+    if int(os.environ.get("MXKV_FUZZ_SEEDS", "0")) <= 0:
+        g = np.load(os.path.join(HERE, "golden", "tree_topology_draw.npz"))
+        cases = [(g["case_%d_W" % i], float(g["case_%d_alpha" % i]), bool(g["case_%d_backtrack" % i]),
+                  None if "case_%d_fails" % i in g.files else (g["case_%d_topo" % i], g["case_%d_scan" % i]))
+                 for i in range(int(g["n_cases"]))]
+        assert len(cases) == 45
+    else:
+        if O.ref_topology_lib() is None:
+            pytest.skip("fresh draws need oracle/_ref/libkvref_topo.so")
+        rng = np.random.default_rng(int.from_bytes(os.urandom(4), "little"))
+        cases = []
+        for n in (2, 3, 4, 5, 6, 7, 8, 9, 11, 13, 16):
+            for rep in range(3):
+                u = rng.uniform(0, 1, (n, n))
+                W = np.where(u < 0.33, 1.0, np.where(u < 0.66, 2.0, 3.0))
+                if rep % 3 == 2:
+                    W = np.where(rng.uniform(0, 1, (n, n)) < 0.3, 0.0, W)
+                W = np.triu(W, 1)
+                W = (W + W.T).astype(np.float32)
+                alpha = float(rng.choice([0.7, 0.5, 0.9]))
+                for bt in ((False, True) if n <= 5 else (False,)):
+                    cases.append((W, alpha, bt, O.ref_compute_trees(W, alpha, bt)))
+    for W, alpha, bt, want in cases:
+        if want is None:
+            with pytest.raises(mx.MXNetError):
+                T.compute_trees(W, alpha, bt)
+            continue
+        topo, scan, _ = T.compute_trees(W, alpha, bt)
+        assert np.array_equal(topo, want[0]) and np.array_equal(scan, want[1]), (W.shape[0], bt, W.tolist())
 
 
 # ---- tests/cpp/kvstore/gpu_topology_test.cc, case by case -------------------------------------------------------

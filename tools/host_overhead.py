@@ -7,7 +7,7 @@ simulated CUDA runtime with kernel launches turned into no-ops -- no GPU needed:
 
 Launches are asynchronous on a real GPU, so this cost is hidden as long as it stays below the kernel time of
 the same call; when it does not (hundreds of small keys, several GPUs driven by one process) the step becomes
-host-bound.  Numbers of this round: profiles/r01_host_overhead.txt."""
+host-bound."""
 import os
 import sys
 import time

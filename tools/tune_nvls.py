@@ -111,13 +111,13 @@ def main():
                 mx.kv.set_nvls(1)
             else:
                 mx.kv.set_nvls(2)
-                grids = [int(x) for x in os.environ.get("TUNE_GRIDS", "0,148,96,64,48,32,24,16").split(",")]
+                grids = [int(x) for x in os.environ.get("TUNE_GRIDS", "0,132,96,64,48,32,24,16").split(",")]
                 quick = bool(os.environ.get("TUNE_QUICK"))      # the default configuration only
                 for threads in ((512,) if quick else (512, 256)):
                     for pipe in ((0,) if quick else (0, 1)):
                         for unroll in ((2,) if quick else (1, 2, 4, 8)):
                             for grid in grids:
-                                if threads == 256 and grid not in (0, 148, 32):
+                                if threads == 256 and grid not in (0, 132, 32):
                                     continue
                                 mx.kv.set_nvls_tuning(unroll=unroll, pipe=pipe, grid=grid, threads=threads)
                                 n0 = mx.kv.launch_count("nvls")
