@@ -70,14 +70,31 @@ struct alignas(16) TensorWork {
   float eta;         // AdamW schedule multiplier
   int n_src;
   int n_out;
-  int pad_;          // bit 0: every pointer 16-byte aligned; bit 1: eligible for the staged variant
+  int flags;         // kWork* bits (WorkFlags)
   union {
     int n_mc;            // NVLS launches: the last n_mc entries of out[] are multicast addresses
     uint32_t tree_prog;  // ORDER_TREE launches (never NVLS): when to add which partial sums, src[] being in the
   };                     //   tree's leaf order (topology.h: ReduceProgram)
-  int reserved_;     // host side only: the key this entry belongs to
+  int key;           // host side only: the key this entry belongs to
 };
 static_assert(sizeof(TensorWork) == 400, "TensorWork layout");
+
+constexpr int kWorkVec16 = 1;    // every pointer 16-byte aligned and begin % 8 == 0: 16-byte packet loads / stores
+constexpr int kWorkStaged = 2;   // eligible for the shared-memory staged variant (implies kWorkVec16)
+
+// The flags of a filled-in entry: kWorkVec16 from its own pointers and range, kWorkStaged where the caller
+// allows it (that depends on dtype, key size and optimizer, which the entry does not carry).  An empty range
+// touches no element, so where it begins does not count: the empty trailing shard of a two-shot key (begin = size)
+// must not take its launch class off the staged kernel, a decision every rank has to make alike.
+inline int WorkFlags(const TensorWork& t, bool staged) {
+  uintptr_t low = t.begin < t.end ? static_cast<uintptr_t>(t.begin) & 7 : 0;
+  for (int k = 0; k < t.n_src; ++k) low |= reinterpret_cast<uintptr_t>(t.src[k]) & 15;
+  for (int k = 0; k < t.n_out; ++k) low |= reinterpret_cast<uintptr_t>(t.out[k]) & 15;
+  low |= (reinterpret_cast<uintptr_t>(t.w) | reinterpret_cast<uintptr_t>(t.w32) | reinterpret_cast<uintptr_t>(t.s0) |
+          reinterpret_cast<uintptr_t>(t.s1)) & 15;
+  if (low != 0) return 0;
+  return kWorkVec16 | (staged ? kWorkStaged : 0);
+}
 
 struct SyncArgs {
   uint32_t* self;                // this rank's signal pad

@@ -103,13 +103,14 @@ void KVStore::AppendTreeWorks(const TensorWork& tw, const TreePlan& tp, bool sli
     TensorWork t = tw;
     for (int k = 0; k < rp.n; ++k) t.src[k] = tw.src[rp.leaf[k]];
     t.tree_prog = rp.prog;
-    t.pad_ &= ~2;
+    t.flags &= ~kWorkStaged;
     // the vector path wants its first element on a packet boundary: a slice that begins inside a packet is led
     // in by a few scalar elements
     const int64_t aligned = std::min<int64_t>(pe, (pb + 7) / 8 * 8);
     if (pb < aligned) {
       TensorWork h = t;
-      h.begin = pb; h.end = aligned; h.pad_ &= ~1;
+      h.begin = pb; h.end = aligned;
+      h.flags = WorkFlags(h, false);
       out->push_back(h);
       pb = aligned;
     }
@@ -759,7 +760,7 @@ void KVStore::BroadcastFromRank0(KeyState& ks, Replica& r) {
   tw.out[0] = r.local.data();
   tw.n_out = 1;
   tw.begin = 0; tw.end = r.local.size();
-  tw.pad_ = 1 | ((r.local.dtype() == kFloat32 && r.local.size() % 4 == 0) ? 2 : 0);
+  tw.flags = WorkFlags(tw, r.local.dtype() == kFloat32 && r.local.size() % 4 == 0);
   std::vector<int> part_dev(pg->world(), pg->dev());
   std::vector<std::vector<TensorWork>> per_part(pg->world());
   per_part[pg->rank()].push_back(tw);
@@ -939,13 +940,14 @@ int64_t ShardLen(int64_t size, int world) {
   return (shard + 127) / 128 * 128;
 }
 
-namespace {
-struct Dest {
+struct KVStore::Dest {
   void* ptr[kMaxRanks];   // address as seen by participant p (MP: peer mapping; SP: same everywhere)
   int owner;              // participant index that owns the memory, -1: none, -2: one copy per rank (MP)
   bool own_only = false;  // two-shot: only the owning participant writes (its own shard of its own copy)
   void* mc = nullptr;     // NVSwitch multicast alias of all copies (one store reaches every rank)
 };
+
+namespace {
 struct PostCopy { NDArray src; NDArray dst; };
 inline bool Overlap(const void* a, size_t an, const void* b, size_t bn) {
   const char* x = static_cast<const char*>(a);
@@ -1126,8 +1128,7 @@ bool KVStore::HostPipelined(std::vector<Group>& groups, bool write_outs) {
       CUDA_CALL(cudaEventRecord(d.ev_h2d[slot], d.copy_in));
       // stage 2: fused reduce(+update) on the element range [b, e)
       CUDA_CALL(cudaStreamWaitEvent(d.stream, d.ev_h2d[slot], 0));
-      TensorWork tw;
-      std::memset(&tw, 0, sizeof(tw));
+      TensorWork tw = ReplicaWork(ks, *r, mp, b, e, lr, wd);
       if (coll) {               // rank q's slot as mapped here; the start rendezvous orders it after q's H2D
         tw.n_src = world;
         for (int q = 0; q < world; ++q)
@@ -1138,13 +1139,7 @@ bool KVStore::HostPipelined(std::vector<Group>& groups, bool write_outs) {
           tw.src[k] = static_cast<char*>(d.host_stage[slot]) + k * slot_stride - static_cast<size_t>(b) * esize;
       }
       tw.out[tw.n_out++] = r->local.data();
-      tw.w = r->local.data();
-      tw.w32 = mp ? static_cast<float*>(r->w32.data()) : nullptr;
-      tw.s0 = r->s0.is_none() ? nullptr : static_cast<float*>(r->s0.data());
-      tw.s1 = r->s1.is_none() ? nullptr : static_cast<float*>(r->s1.data());
-      tw.begin = b; tw.end = e;
-      tw.lr = lr; tw.wd = wd; tw.eta = KeyEta(ks); tw.reserved_ = ks.key;
-      tw.pad_ = 1 | ((esize == 4 && ks.size % 4 == 0) ? 2 : 0);
+      tw.flags = WorkFlags(tw, esize == 4 && ks.size % 4 == 0);
       std::vector<std::vector<TensorWork>> per_part(world);
       per_part[me].push_back(tw);
       // (the end rendezvous of a collective launch also tells this rank that no peer still reads its slot)
@@ -1278,8 +1273,7 @@ void KVStore::ReduceUpdateCompressed(std::vector<Group>& groups, bool write_outs
       float* deq = nullptr;
       CUDA_CALL(cudaMallocAsync(reinterpret_cast<void**>(&deq), static_cast<size_t>(n_total) * std::max<int64_t>(ks.size, 4) * 4, s));
       temps.push_back({deq, dev});
-      TensorWork tw;
-      std::memset(&tw, 0, sizeof(tw));
+      TensorWork tw = ReplicaWork(ks, r, mp, 0, ks.size, lr, wd);
       tw.n_src = n_total;
       for (int k = 0; k < n_total; ++k) {
         const uint32_t* codes;
@@ -1300,7 +1294,6 @@ void KVStore::ReduceUpdateCompressed(std::vector<Group>& groups, bool write_outs
         tw.src[k] = out;
       }
       tw.out[tw.n_out++] = stage_only ? hier_base_.at(ks.key) : r.local.data();
-      bool vec_ok = (ks.size % 4 == 0);          // scratch slices stay 16-byte aligned only then
       if (write_outs) {
         for (NDArray* o : g.outs) {
           MXKV_CHECK(o->size() == ks.size && o->dtype() == ks.dtype) << "pushpull: output does not match key " << ks.key;
@@ -1308,18 +1301,11 @@ void KVStore::ReduceUpdateCompressed(std::vector<Group>& groups, bool write_outs
           if (oc.is_gpu() && oc.dev_id == dev && tw.n_out < kMaxOut &&
               !(groups.size() > 1 && alias.OverlapsOther(o->data(), o->nbytes(), static_cast<int>(gi)))) {
             tw.out[tw.n_out++] = o->data();
-            vec_ok = vec_ok && ((reinterpret_cast<uintptr_t>(o->data()) & 15) == 0);
             written.insert(o);
           }
         }
       }
-      tw.w = r.local.data();
-      tw.w32 = mp ? static_cast<float*>(r.w32.data()) : nullptr;
-      tw.s0 = r.s0.is_none() ? nullptr : static_cast<float*>(r.s0.data());
-      tw.s1 = r.s1.is_none() ? nullptr : static_cast<float*>(r.s1.data());
-      tw.begin = 0; tw.end = ks.size;
-      tw.lr = lr; tw.wd = wd; tw.eta = KeyEta(ks); tw.reserved_ = ks.key;
-      tw.pad_ = vec_ok ? 3 : 0;
+      tw.flags = ks.size % 4 == 0 ? WorkFlags(tw, true) : 0;   // (other sizes keep the scalar path)
       LaunchLocal(LaunchClassKey{SYNC_NONE, ks.dtype, mp ? 1 : 0}, tw, opt_kind, dev);
       if (!stage_only) r.fresh = true;
     }
@@ -1498,7 +1484,9 @@ bool KVStore::TryReplayRaw(int kind, uint32_t vnum, const int* vkeys, NDArray* c
   if (plan_mode_ == 1 && it != plans_.end() && it->second.recorded && it->second.sig == sig &&
       PlanEpochsMatch(it->second)) {
     if (key_type_ == kUndefinedKey) key_type_ = kIntKey;
-    PlanReplay(it->second);
+    PlanPatch(it->second, true);
+    IssuePlan(it->second);
+    plan_hits_++;
     raw_pending_ = false;
     return true;
   }
@@ -1533,18 +1521,64 @@ void KVStore::PlanPatch(CallPlan& p, bool commit_counts) {
       }
 }
 
-void KVStore::PlanReplay(CallPlan& p) {
+// Everything a dense call enqueues, in this order; a fresh call runs it once its plan is built, a repeated call
+// after PlanPatch.
+void KVStore::IssuePlan(CallPlan& p) {
   Runtime* rt = Runtime::Get();
   for (int dev : p.touched) rt->AcquireUser(dev);
-  PlanPatch(p, true);
   for (auto& w : p.pre_waits) rt->StreamWait(w.first, w.second);
   for (auto& c : p.pre_copies) CopyFromTo(c.first, c.second);
-  for (auto& l : p.launches) LaunchWorks(l.ck, l.per_part, l.busiest, p.opt_kind, p.part_dev);
+  for (auto& s : p.staged) CopyBytes(s.src.data(), s.src.ctx(), s.tmp, Context{kGPU, s.dev}, s.src.nbytes());
+  if (IsNormOpt(p.opt_kind)) {
+    // all classes together: the phases of every class are interleaved so that the overflow check
+    // covers the whole push
+    std::vector<NormClass> all;
+    for (auto& l : p.launches) all.push_back(NormClass{l.ck, &l.per_part, &l.busiest});
+    LaunchNormWorks(all, p.opt_kind, p.part_dev);
+  } else {
+    for (auto& l : p.launches) LaunchWorks(l.ck, l.per_part, l.busiest, p.opt_kind, p.part_dev);
+  }
+  for (auto& s : p.staged) {
+    DeviceGuard dg(s.dev);
+    CUDA_CALL(cudaFreeAsync(s.tmp, rt->Dev(s.dev).stream));
+  }
+  // destinations on other GPUs were written by the root's kernel
   if (!p.collective)
     for (int dev : p.touched) if (dev != p.root_dev) rt->StreamWait(dev, p.root_dev);
+  if (!p.callback_keys.empty()) {
+    ProcessGroup* pg = PG();
+    for (KeyState* ks : p.callback_keys) RunCallbackUpdater(*ks, *FindReplica(*ks, p.part_dev[pg ? pg->rank() : 0]));
+  }
   for (auto& c : p.post_copies) CopyFromTo(c.first, c.second);
   for (int dev : p.touched) rt->ReleaseToUser(dev);
-  plan_hits_++;
+}
+
+// MXKV_B200_PLAN=2: the replay of a kept plan must issue exactly what the full path builds
+bool KVStore::SamePlan(const CallPlan& a, const CallPlan& b) const {
+  auto same_copies = [](const std::vector<std::pair<NDArray, NDArray>>& x,
+                        const std::vector<std::pair<NDArray, NDArray>>& y) {
+    if (x.size() != y.size()) return false;
+    for (size_t i = 0; i < x.size(); ++i)
+      if (x[i].first.data() != y[i].first.data() || x[i].second.data() != y[i].second.data()) return false;
+    return true;
+  };
+  if (a.launches.size() != b.launches.size() || a.part_dev != b.part_dev || a.touched != b.touched ||
+      a.pre_waits != b.pre_waits || !same_copies(a.pre_copies, b.pre_copies) ||
+      !same_copies(a.post_copies, b.post_copies) || a.opt_kind != b.opt_kind || a.fused != b.fused ||
+      a.collective != b.collective || a.root_dev != b.root_dev || a.repeatable != b.repeatable ||
+      a.staged.size() != b.staged.size() || a.callback_keys.size() != b.callback_keys.size())
+    return false;
+  for (size_t i = 0; i < a.launches.size(); ++i) {
+    const PlanLaunch& x = a.launches[i];
+    const PlanLaunch& y = b.launches[i];
+    if (x.ck < y.ck || y.ck < x.ck || x.busiest != y.busiest || x.per_part.size() != y.per_part.size()) return false;
+    for (size_t q = 0; q < x.per_part.size(); ++q)
+      if (x.per_part[q].size() != y.per_part[q].size() ||
+          (!x.per_part[q].empty() &&
+           std::memcmp(x.per_part[q].data(), y.per_part[q].data(), x.per_part[q].size() * sizeof(TensorWork)) != 0))
+        return false;
+  }
+  return true;
 }
 
 void KVStore::PlaceKey(const Group& g, KeyState& ks, std::vector<int>* devs_out, std::vector<int>* key_part_out,
@@ -1593,6 +1627,34 @@ void KVStore::PlaceKey(const Group& g, KeyState& ks, std::vector<int>* devs_out,
   *key_collective_out = key_collective;
 }
 
+namespace {
+void Touch(std::vector<int>* touched, int dev) {
+  if (dev >= 0 && std::find(touched->begin(), touched->end(), dev) == touched->end()) touched->push_back(dev);
+}
+}  // namespace
+
+// One key of a dense call while ReduceUpdate builds the call's plan: each stage fills in what the next needs.
+struct KVStore::KeyBuild {
+  const std::vector<Group>& groups;
+  size_t gi;                        // this key's group (and its index in CallPlan::keys)
+  bool write_outs;
+  const AliasIndex& alias;
+  KeyState& ks;
+  int first = 0, last = 0;          // local participant slots
+  std::vector<int> devs;            // per source: device, -1 = host (PlaceKey)
+  std::vector<Replica*> rep;        // per participant slot, the local ones only (KeyReplicas)
+  bool mp = false;                  // fp32 master weight
+  bool two_shot = false;            // sharded over the participants
+  const TreePlan* tree = nullptr;   // MXNET_KVSTORE_USETREE (KeyTree)
+  bool tree_sliced = false;
+  bool nvls = false;                // the switch sums and stores (KeyDests)
+  const Group& g() const { return groups[gi]; }
+};
+
+// Ordering: nothing below issues an operation that reads or writes a caller array.  The build only enqueues work on
+// engine-owned memory (EnsureReplica / EnsureState / SyncState / GatherLocal / GatherState); stream waits, staging
+// copies (also those into temporaries) and the launches are plan steps that IssuePlan runs after it has acquired
+// every device of the call, once.
 void KVStore::ReduceUpdate(std::vector<Group>& groups, bool write_outs) {
   // an overflow of the previous step is settled before this step's update counts are taken
   if (hier_phase_ == 0 && opt_.enabled && updater_ == nullptr && opt_.skip_nonfinite) ResolveOverflow();
@@ -1600,8 +1662,8 @@ void KVStore::ReduceUpdate(std::vector<Group>& groups, bool write_outs) {
   // (multi-node with compression: phase 1 is the compressed reduce, phase 2 the ordinary update from the slices)
   if (gc_bits_ != 0 && hier_phase_ != 2) { ReduceUpdateCompressed(groups, write_outs); return; }
 
-  // ---- a repeated call: replay its recorded work lists (only counts and lr / wd / eta are new) ------------
-  CallPlan rec;                         // what this call would record
+  // ---- a repeated call: the plan of the last identical call is kept (only counts and lr / wd / eta are new) ----
+  CallPlan plan;
   bool rec_on = false, rec_repeat = false;
   uint64_t rec_hash = 0;
   std::unique_ptr<CallPlan> verify;     // MXKV_B200_PLAN=2: the plan as a replay would have patched it
@@ -1609,12 +1671,12 @@ void KVStore::ReduceUpdate(std::vector<Group>& groups, bool write_outs) {
       !(opt_.enabled && IsNormOpt(opt_.kind))) {
     raw_pending_ = false;               // (consumed: a recursive or later call must not record under it)
     rec_on = true;
-    rec.sig = raw_sig_;
+    plan.sig = raw_sig_;
     rec_hash = raw_hash_;
     auto it = plans_.find(rec_hash);
-    if (it != plans_.end() && it->second.sig == rec.sig && PlanEpochsMatch(it->second)) {
+    if (it != plans_.end() && it->second.sig == plan.sig && PlanEpochsMatch(it->second)) {
       if (it->second.recorded) {        // (MXKV_B200_PLAN=1 replays in TryReplayRaw and never gets here)
-        // verify mode: run the full path below and compare what it builds
+        // verify mode: build the plan below and compare
         verify.reset(new CallPlan(it->second));
         PlanPatch(*verify, false);
       }
@@ -1622,13 +1684,13 @@ void KVStore::ReduceUpdate(std::vector<Group>& groups, bool write_outs) {
     }
   }
   if (hier_phase_ == 0 && HostPipelined(groups, write_outs)) return;
-  Runtime* rt = Runtime::Get();
   ProcessGroup* pg = PG();
   const bool mp_mode = pg != nullptr;
   const bool callback = updater_ != nullptr && hier_phase_ != 1;
   // multi-node: phase 1 only sums the node's values into the staging slices; phase 2 is the ordinary path with
   // the (by then globally summed) slice as the only source
-  const bool fused = opt_.enabled && !callback && hier_phase_ != 1;
+  plan.fused = opt_.enabled && !callback && hier_phase_ != 1;
+  plan.opt_kind = plan.fused ? opt_.kind : OPT_NONE;
 
   // Keys of one call that reduce on different GPUs (e.g. host-resident values for keys whose stored
   // values live on different GPUs) are served group by group; the reference has no such restriction
@@ -1666,35 +1728,11 @@ void KVStore::ReduceUpdate(std::vector<Group>& groups, bool write_outs) {
     }
   }
 
-  // participant slot -> device; SP: discovered from the first key, MP: this rank only is local
-  struct LaunchClass {
-    std::vector<std::vector<TensorWork>> per_part;   // [participant] -> work list
-    std::vector<int64_t> busiest;                    // per key: elements the busiest rank handles
-  };
-  std::map<LaunchClassKey, LaunchClass> classes;
-  std::vector<int> part_dev;      // device of participant p (SP) / own device at index rank (MP)
-  std::vector<PostCopy> post;
-  std::vector<void*> temps;       // cudaMallocAsync'ed staging, freed after the launches
-  std::vector<int> temp_dev;
-  std::set<int> touched;
-  std::vector<KeyState*> callback_keys;
-  auto touch = [&](int dev) { if (dev >= 0 && touched.insert(dev).second) rt->AcquireUser(dev); };
-  bool rec_bad = false;                 // this call did something a replay could not (temporaries, layout changes)
-  auto stream_wait = [&](int waiter, int signaler) {
-    rt->StreamWait(waiter, signaler);
-    if (waiter != signaler) rec.pre_waits.emplace_back(waiter, signaler);
-  };
-
-  int n_part = 0;
-  bool collective = false;
-  int root_dev = -1;
   const AliasIndex alias(groups);
-
   for (size_t gi = 0; gi < groups.size(); ++gi) {
     Group& g = groups[gi];
     KeyState& ks = GetKey(g.key);
     MXKV_CHECK(ks.stype == kDefaultStorage) << "key " << g.key << " is row_sparse; dense push not allowed";
-    const size_t esize = DTypeSize(ks.dtype);
     const int n_src = static_cast<int>(g.vals.size());
     MXKV_CHECK(n_src >= 1 && n_src <= kMaxSrc) << "push of " << n_src << " values for one key (max " << kMaxSrc << ")";
     for (auto& v : g.vals) {
@@ -1703,429 +1741,364 @@ void KVStore::ReduceUpdate(std::vector<Group>& groups, bool write_outs) {
       MXKV_CHECK(v.dtype() == ks.dtype) << "push: dtype mismatch for key " << ks.key
                                         << " (Only support input/output with the same data type)";
     }
-
-    // ---- placement ------------------------------------------------------
-    std::vector<int> devs;        // per source; -1 = host
+    KeyBuild k{groups, gi, write_outs, alias, ks};
     std::vector<int> key_part;    // participant devices for this key
     bool key_collective = false;
-    PlaceKey(g, ks, &devs, &key_part, &key_collective);
+    PlaceKey(g, ks, &k.devs, &key_part, &key_collective);
     if (gi == 0) {
-      part_dev = key_part; n_part = static_cast<int>(key_part.size()); collective = key_collective;
-      root_dev = key_part[0];
+      plan.part_dev = key_part; plan.collective = key_collective; plan.root_dev = key_part[0];
     } else {
-      MXKV_CHECK(key_part == part_dev && key_collective == collective)
+      MXKV_CHECK(key_part == plan.part_dev && key_collective == plan.collective)
           << "all keys of one push/pushpull call must use the same set of devices";
     }
-    const int my_first = mp_mode ? pg->rank() : 0;
-    const int my_last = mp_mode ? pg->rank() : n_part - 1;
-
-    // ---- replicas -------------------------------------------------------
-    std::vector<Replica*> rep(n_part, nullptr);
-    for (int p = my_first; p <= my_last; ++p) {
-      touch(part_dev[p]);
-      rep[p] = &EnsureReplica(ks, part_dev[p]);
-    }
-    // EnsureReplica may reallocate ks.reps: re-resolve pointers
-    for (int p = my_first; p <= my_last; ++p) rep[p] = FindReplica(ks, part_dev[p]);
-
-    const bool lowp = ks.dtype == kFloat16 || ks.dtype == kBfloat16;
-    const bool mp = fused && (opt_.multi_precision || lowp);
-    if (fused) {
-      MXKV_CHECK(ks.dtype == kFloat32 || lowp) << "fused optimizers need float32/float16/bfloat16 keys";
-      for (int p = my_first; p <= my_last; ++p) EnsureState(ks, *rep[p], mp);
-    }
-
-    const bool two_shot = collective && !hier_whole_keys_ &&
-                          static_cast<int64_t>(ks.size * esize) >= rt->twoshot_bytes &&
-                          ks.size >= static_cast<int64_t>(n_part) * 128;
-    if (hier_phase_ != 1 && ks.local_world > 0 &&
-        (callback || !(two_shot && ks.local_world == n_part && ks.shard_devs == part_dev))) {
-      GatherLocal(ks);
-      rec_bad = true;
-      for (int p = my_first; p <= my_last; ++p) rep[p] = &EnsureReplica(ks, part_dev[p]);
-      for (int p = my_first; p <= my_last; ++p) rep[p] = FindReplica(ks, part_dev[p]);
-    }
-    if (fused) {
-      // the optimizer state is laid out for this call's shape: sharded over the n participants of a
-      // two-shot push, complete on every replica otherwise (also when a key that used to be sharded is
-      // now pushed from one GPU only)
-      const int want = (collective && two_shot) ? n_part : 0;
-      const bool same = ks.state_world == want && (want == 0 || ks.state_devs == part_dev);
-      if (ks.count > 0 && !same) { GatherState(ks); rec_bad = true; }
-      ks.state_world = want;
-      if (want > 0) ks.state_devs = part_dev; else ks.state_devs.clear();
-      // a replica that sat out earlier updates (its GPU did not take part) first takes over the state of
-      // one that did; after this call only the participants' state is current
-      for (int p = my_first; p <= my_last; ++p) SyncState(ks, *rep[p]);
-      for (auto& r : ks.reps) {
-        bool part = false;
-        for (int p = my_first; p <= my_last; ++p) part = part || (&r == rep[p]);
-        if (!part) r.state_fresh = false;
-      }
-    }
-
-    // ---- sources as addressable pointers ----------------------------------
-    // srcptr[p][k]: address of source k for the kernel running as participant p
-    std::vector<std::vector<const void*>> srcptr(n_part, std::vector<const void*>(collective ? n_part : n_src));
-    if (mp_mode && hier_phase_ == 2) {
-      srcptr[pg->rank()].assign(1, hier_base_.at(ks.key));
-    } else if (mp_mode) {
-      const NDArray& v = g.vals[0];
-      NDArray sym_src;
-      if (v.symmetric() && collective) {
-        sym_src = v;
-      } else if (collective) {
-        Replica& r = *rep[pg->rank()];
-        if (r.stage.is_none()) r.stage = NDArray::Empty(ks.shape, Context{kGPU, pg->dev()}, ks.dtype, true);
-        CopyFromTo(v, r.stage);                       // D2D or H2D
-        rec.pre_copies.emplace_back(v, r.stage);
-        sym_src = r.stage;
-      }
-      if (collective) {
-        for (int k = 0; k < n_part; ++k) srcptr[pg->rank()][k] = sym_src.peer_data(k);
-      } else {
-        if (devs[0] < 0) {
-          void* t = nullptr;
-          DeviceGuard dg(pg->dev());
-          CUDA_CALL(cudaMallocAsync(&t, v.nbytes() ? v.nbytes() : 16, rt->Dev(pg->dev()).stream));
-          temps.push_back(t); temp_dev.push_back(pg->dev()); rec_bad = true;
-          CopyBytes(v.data(), v.ctx(), t, Context{kGPU, pg->dev()}, v.nbytes());
-          srcptr[pg->rank()][0] = t;
-        } else {
-          srcptr[pg->rank()][0] = v.data();
-        }
-      }
-    } else if (collective) {
-      for (int p = 0; p < n_part; ++p)
-        for (int k = 0; k < n_part; ++k) srcptr[p][k] = g.vals[k].data();
-    } else {
-      for (int k = 0; k < n_src; ++k) {
-        const NDArray& v = g.vals[k];
-        const bool direct = devs[k] == root_dev || (devs[k] >= 0 && (rt->EnablePeerAccess({root_dev, devs[k]}),
-                                                                   rt->PeerOK(root_dev, devs[k])));
-        if (direct) {
-          if (devs[k] != root_dev) {              // foreign GPU read by the root kernel
-            touch(devs[k]);
-            stream_wait(root_dev, devs[k]);
-          }
-          srcptr[0][k] = v.data();
-        } else {                                   // host value, or no P2P: stage on the root
-          if (devs[k] >= 0) touch(devs[k]);
-          void* t = nullptr;
-          {
-            DeviceGuard dg(root_dev);
-            CUDA_CALL(cudaMallocAsync(&t, v.nbytes() ? v.nbytes() : 16, rt->Dev(root_dev).stream));
-          }
-          temps.push_back(t); temp_dev.push_back(root_dev); rec_bad = true;
-          CopyBytes(v.data(), v.ctx(), t, Context{kGPU, root_dev}, v.nbytes());
-          srcptr[0][k] = t;
-        }
-      }
-    }
-
-    // ---- MXNET_KVSTORE_USETREE: which tree(s) this key's sum goes up ------------------------------------
-    // Two values add the same way in any order, and the integer dtypes wrap: only three or more floating-point
-    // values are order-sensitive.  Host-resident values and multi-node stores keep the plain order (the
-    // reference's tree needs every value on its own GPU, comm_tree.h:108-121).
-    const TreePlan* tree_plan = nullptr;
-    bool tree_sliced = false;
-    if (tree_ && collective && n_part >= 3 && hier_phase_ == 0 &&
-        (ks.dtype == kFloat32 || ks.dtype == kFloat16 || ks.dtype == kBfloat16 || ks.dtype == kFloat64)) {
-      MXKV_CHECK(!(fused && IsNormOpt(opt_.kind)))
-          << "MXNET_KVSTORE_USETREE=1: the layer-wise optimizers (LAMB / LANS / LARS) are not served in tree order";
-      MXKV_CHECK(TreeKernelAvailable(ks.dtype, fused ? opt_.kind : OPT_NONE, mp ? 1 : 0))
-          << "MXNET_KVSTORE_USETREE=1: no tree kernel for dtype " << ks.dtype << " with optimizer kind " << opt_.kind;
-      tree_plan = &TreePlanFor(mp_mode ? pg->rank_devs() : part_dev);
-      const int64_t rows = ks.shape.empty() ? 1 : ks.shape[0];
-      tree_sliced = ks.size > tree_bound_ && rows >= 2 * static_cast<int64_t>(n_part);
-    }
-
-    // ---- destinations -------------------------------------------------------
-    bool nvls_key = false;
-    std::vector<Dest> dests;
-    auto add_dest_sp = [&](void* ptr, int dev) {
-      Dest d;
-      for (int p = 0; p < kMaxRanks; ++p) d.ptr[p] = ptr;
-      d.owner = -1;
-      for (int p = 0; p < n_part; ++p) if (part_dev[p] == dev) d.owner = p;
-      dests.push_back(d);
-    };
-    if (callback) {
-      Replica& root = *rep[my_first];
-      if (root.merged.is_none())
-        root.merged = NDArray::Empty(ks.shape, Context{kGPU, root.dev}, ks.dtype, mp_mode);
-      if (mp_mode && collective) {
-        Dest d; d.owner = -2;   // every rank owns its own copy
-        for (int p = 0; p < n_part; ++p) d.ptr[p] = root.merged.peer_data(p);
-        dests.push_back(d);
-      } else {
-        add_dest_sp(root.merged.data(), root.dev);
-      }
-      callback_keys.push_back(&ks);
-    } else {
-      // which outputs can be written by the kernel itself?
-      std::vector<char> out_direct(g.outs.size(), 0);
-      bool need_post = false;
-      if (write_outs) {
-        int budget = kMaxOut - 1 - (mp_mode ? 1 : static_cast<int>(ks.reps.size()));
-        for (size_t oi = 0; oi < g.outs.size(); ++oi) {
-          NDArray* o = g.outs[oi];
-          MXKV_CHECK(o->size() == ks.size && o->dtype() == ks.dtype)
-              << "pushpull: output does not match key " << ks.key;
-          const Context oc = o->ctx();
-          bool direct = false;
-          if (oc.is_gpu() && budget > 0) {
-            if (mp_mode) {
-              direct = collective ? o->symmetric() : (oc.dev_id == pg->dev());
-            } else {
-              for (int p = 0; p < n_part; ++p) if (part_dev[p] == oc.dev_id) direct = true;
-            }
-            // one-shot in-place allreduce: peers still read this buffer while we would write it
-            if (direct && collective && !two_shot) {
-              for (auto& v : g.vals)
-                if (Overlap(o->data(), o->nbytes(), v.data(), v.nbytes())) direct = false;
-            }
-            if (direct && !Aligned16(o->data())) direct = false;
-            if (direct && groups.size() > 1 && alias.OverlapsOther(o->data(), o->nbytes(), static_cast<int>(gi)))
-              direct = false;
-          }
-          out_direct[oi] = direct ? 1 : 0;
-          if (direct) --budget; else need_post = true;
-        }
-      }
-      // Two-shot keys keep the stored value sharded (rank p owns shard p of its own replica) unless
-      // an output has to be copied out of a complete replica afterwards: the all-gather then moves
-      // each shard over NVLink once per peer (into the outputs) instead of twice.
-      // NVLS: every array of the key is bound to a multicast object (and nothing has to be copied
-      // out of a complete replica afterwards)
-      // (auto: above 4 ranks.  Per direction the switch path moves S(1 + 1/n) against 2S(n-1)/n of
-      // the peer path: 1.5x more at n=2, 1.2x less at n=4 -- where the peer path is still kept because
-      // it is bit-exact --, 1.56x less at n=8)
-      if (mp_mode && collective && !hier_ && tree_plan == nullptr &&
-          (rt->nvls_mode >= 2 || (rt->nvls_mode == 1 && n_part > 4)) &&
-          !(fused && IsNormOpt(opt_.kind)) && ks.dtype == kFloat32 && ks.size % 4 == 0 &&
-          g.vals[0].mc_data() != nullptr && Aligned16(g.vals[0].mc_data()) && !(two_shot && need_post)) {
-        nvls_key = true;
-        if (write_outs)
-          for (size_t oi = 0; oi < g.outs.size(); ++oi)
-            if (out_direct[oi] && g.outs[oi]->mc_data() == nullptr) nvls_key = false;
-      }
-      const bool shard_local = two_shot && !need_post;
-      if (hier_phase_ == 1) {
-        // the node's sum of this rank's range (the whole key when it is not sharded) goes to the staging slice
-        Dest d; d.owner = collective ? -2 : -1; d.own_only = shard_local;
-        for (int p = 0; p < kMaxRanks; ++p) d.ptr[p] = hier_base_.at(ks.key);
-        if (!collective) d.owner = 0;
-        dests.push_back(d);
-      } else if (mp_mode && collective) {
-        Dest d; d.owner = -2; d.own_only = shard_local;
-        for (int p = 0; p < n_part; ++p) d.ptr[p] = rep[pg->rank()]->local.peer_data(p);
-        dests.push_back(d);
-      } else {
-        for (auto& r : ks.reps) {
-          const bool reachable = r.dev == root_dev || collective ||
-                                 (rt->EnablePeerAccess({root_dev, r.dev}), rt->PeerOK(root_dev, r.dev));
-          bool is_part = false;
-          for (int p = 0; p < n_part; ++p) if (part_dev[p] == r.dev) is_part = true;
-          if (is_part || (reachable && !collective)) {
-            if (!is_part) { touch(r.dev); stream_wait(root_dev, r.dev); }
-            add_dest_sp(r.local.data(), r.dev);
-            dests.back().own_only = shard_local;
-            r.fresh = true;
-          } else {
-            r.fresh = false;          // refreshed lazily by EnsureReplica
-          }
-        }
-      }
-      if (hier_phase_ == 1) {
-        // the stored value is not touched in this phase
-      } else if (shard_local) { ks.local_world = n_part; ks.shard_devs = part_dev; }
-      else ks.local_world = 0;
-      if (write_outs) {
-        for (size_t oi = 0; oi < g.outs.size(); ++oi) {
-          NDArray* o = g.outs[oi];
-          const Context oc = o->ctx();
-          if (out_direct[oi]) {
-            touch(oc.dev_id);
-            if (mp_mode && collective) {
-              Dest d; d.owner = -2;
-              for (int p = 0; p < n_part; ++p) d.ptr[p] = o->peer_data(p);
-              d.mc = o->mc_data();
-              dests.push_back(d);
-            } else {
-              add_dest_sp(o->data(), oc.dev_id);
-            }
-          } else {
-            if (oc.is_gpu()) touch(oc.dev_id);
-            PostCopy pc;
-            pc.dst = *o;
-            // copy out of a replica this call has just written: a replica on the output's own GPU only if
-            // that GPU took part (a replica left over from an earlier device set is stale now)
-            Replica* near = oc.is_gpu() ? FindReplica(ks, oc.dev_id) : nullptr;
-            const int sdev = (near != nullptr && near->fresh) ? oc.dev_id : part_dev[my_first];
-            pc.src = FindReplica(ks, sdev)->local;
-            post.push_back(pc);
-          }
-        }
-      }
-    }
-    MXKV_CHECK(static_cast<int>(dests.size()) <= kMaxOut) << "too many destinations for key " << ks.key;
-
-    // ---- hyper-parameters -------------------------------------------------
-    float lr = 0.f, wd = 0.f;
-    if (fused) {
-      ks.count += 1;                 // Optimizer._update_count
-      lr = KeyLR(ks);
-      wd = KeyWD(ks);
-    }
-
-    // ---- work entries -------------------------------------------------------
-    // one launch (one pair of rendezvous) for the one-shot and the two-shot keys of a call: the
-    // release/acquire flavour of the end barrier covers both
-    const int sync_mode = !collective ? SYNC_NONE : SYNC_WRITE_PEERS;
-    LaunchClassKey ck{sync_mode, ks.dtype, mp ? 1 : 0};
-    ck.nvls = nvls_key ? 1 : 0;
-    ck.tree = tree_plan != nullptr ? 1 : 0;
-    LaunchClass& lc = classes[ck];
-    auto& cls = lc.per_part;
-    if (cls.empty()) cls.resize(n_part);
-    const int64_t shard = two_shot ? ShardLen(ks.size, n_part) : ks.size;
-    lc.busiest.push_back(std::min<int64_t>(ks.size, shard));
-    for (int p = my_first; p <= my_last; ++p) {
-      TensorWork tw;
-      std::memset(&tw, 0, sizeof(tw));
-      bool vec_ok = true;
-      if (nvls_key) {                  // the switch sums the replicas: one multicast "source"
-        tw.n_src = 1;
-        tw.src[0] = g.vals[0].mc_data();
-      } else {
-        tw.n_src = static_cast<int>(srcptr[p].size());
-        for (int k = 0; k < tw.n_src; ++k) {
-          tw.src[k] = srcptr[p][k];
-          vec_ok = vec_ok && Aligned16(tw.src[k]);
-        }
-      }
-      std::vector<void*> mc_outs;
-      for (auto& d : dests) {
-        if (d.owner == -2) {           // MP: one copy per rank
-          if (two_shot && !d.own_only) {
-            if (nvls_key) { mc_outs.push_back(d.mc); vec_ok = vec_ok && Aligned16(d.mc); continue; }
-            for (int q = 0; q < n_part; ++q) { tw.out[tw.n_out++] = d.ptr[q]; vec_ok = vec_ok && Aligned16(d.ptr[q]); }
-          } else {
-            tw.out[tw.n_out++] = d.ptr[p]; vec_ok = vec_ok && Aligned16(d.ptr[p]);
-          }
-          continue;
-        }
-        bool mine;
-        if (!collective) mine = true;
-        else if (two_shot && !d.own_only) mine = true;
-        else mine = (d.owner == p) || (d.owner == -1 && p == 0);
-        if (mine) { tw.out[tw.n_out++] = d.ptr[p]; vec_ok = vec_ok && Aligned16(d.ptr[p]); }
-      }
-      for (void* m : mc_outs) { tw.out[tw.n_out++] = m; tw.n_mc++; }
-      MXKV_CHECK(tw.n_out <= kMaxOut) << "too many destinations for key " << ks.key;
-      if (nvls_key) MXKV_CHECK(vec_ok) << "NVLS arrays must be 16-byte aligned";
-      Replica& r = *rep[p];
-      tw.w = r.local.data();
-      tw.w32 = mp ? static_cast<float*>(r.w32.data()) : nullptr;
-      tw.s0 = r.s0.is_none() ? nullptr : static_cast<float*>(r.s0.data());
-      tw.s1 = r.s1.is_none() ? nullptr : static_cast<float*>(r.s1.data());
-      if (two_shot) {
-        tw.begin = std::min<int64_t>(ks.size, shard * p);
-        tw.end = std::min<int64_t>(ks.size, shard * (p + 1));
-      } else {
-        tw.begin = 0; tw.end = ks.size;
-      }
-      tw.lr = lr; tw.wd = wd; tw.eta = KeyEta(ks); tw.reserved_ = ks.key;
-      tw.pad_ = (vec_ok ? 1 : 0) | ((vec_ok && esize == 4 && ks.size % 4 == 0) ? 2 : 0);
-      if (tree_plan != nullptr) AppendTreeWorks(tw, *tree_plan, tree_sliced, ks, n_part, &cls[p]);
-      else cls[p].push_back(tw);
-    }
+    k.first = mp_mode ? pg->rank() : 0;
+    k.last = mp_mode ? pg->rank() : static_cast<int>(plan.part_dev.size()) - 1;
+    KeyReplicas(plan, k);
+    const std::vector<std::vector<const void*>> srcptr = KeySources(plan, k);
+    KeyTree(plan, k);
+    const std::vector<Dest> dests = KeyDests(plan, k);
+    KeyWorks(plan, k, srcptr, dests);
+    plan.keys.push_back(g.key);
   }
-
-  // ---- launches: one per class per local participant --------------------------
-  const int opt_kind = fused ? opt_.kind : OPT_NONE;
-  if (rec_on && !callback) {
-    rec.keys.clear();
-    for (auto& g : groups) rec.keys.push_back(g.key);
-    std::unordered_map<int, int> key_pos;
-    for (size_t i = 0; i < rec.keys.size(); ++i) key_pos[rec.keys[i]] = static_cast<int>(i);
-    for (auto& kv : classes) {
-      PlanLaunch pl{kv.first, kv.second.per_part, kv.second.busiest, {}};
-      pl.key_idx.resize(pl.per_part.size());
-      for (size_t q = 0; q < pl.per_part.size(); ++q)
-        for (auto& tw : pl.per_part[q]) pl.key_idx[q].push_back(key_pos.at(tw.reserved_));
-      rec.launches.push_back(std::move(pl));
-    }
-    rec.part_dev = part_dev;
-    rec.touched.assign(touched.begin(), touched.end());
-    for (auto& pc : post) rec.post_copies.emplace_back(pc.src, pc.dst);
-    rec.opt_kind = opt_kind; rec.fused = fused; rec.collective = collective; rec.root_dev = root_dev;
-    if (verify) {
-      // the replay of the recorded plan must be exactly what the full path has just built
-      const CallPlan& v = *verify;
-      bool same = v.launches.size() == rec.launches.size() && v.part_dev == rec.part_dev && v.opt_kind == rec.opt_kind &&
-                  v.fused == rec.fused && v.collective == rec.collective && v.root_dev == rec.root_dev &&
-                  v.pre_waits == rec.pre_waits && v.pre_copies.size() == rec.pre_copies.size() &&
-                  v.post_copies.size() == rec.post_copies.size() && !rec_bad && !temps.size();
-      std::set<int> vt(v.touched.begin(), v.touched.end());
-      same = same && vt == touched;
-      for (size_t i = 0; same && i < v.launches.size(); ++i) {
-        const PlanLaunch& a = v.launches[i];
-        const PlanLaunch& b = rec.launches[i];
-        same = !(a.ck < b.ck) && !(b.ck < a.ck) && a.busiest == b.busiest && a.per_part.size() == b.per_part.size();
-        for (size_t q = 0; same && q < a.per_part.size(); ++q)
-          same = a.per_part[q].size() == b.per_part[q].size() &&
-                 (a.per_part[q].empty() ||
-                  std::memcmp(a.per_part[q].data(), b.per_part[q].data(), a.per_part[q].size() * sizeof(TensorWork)) == 0);
-      }
-      for (size_t i = 0; same && i < v.pre_copies.size(); ++i)
-        same = v.pre_copies[i].first.data() == rec.pre_copies[i].first.data() &&
-               v.pre_copies[i].second.data() == rec.pre_copies[i].second.data();
-      for (size_t i = 0; same && i < v.post_copies.size(); ++i)
-        same = v.post_copies[i].first.data() == rec.post_copies[i].first.data() &&
-               v.post_copies[i].second.data() == rec.post_copies[i].second.data();
-      MXKV_CHECK(same) << "MXKV_B200_PLAN=2: the cached launch plan differs from the work lists of the full path";
-      plan_hits_++;
-    }
+  std::sort(plan.touched.begin(), plan.touched.end());
+  if (verify) {
+    MXKV_CHECK(SamePlan(*verify, plan)) << "MXKV_B200_PLAN=2: the cached launch plan differs from the one the full path builds";
+    plan_hits_++;
   }
-  if (IsNormOpt(opt_kind)) {
-    // all classes together: the phases of every class are interleaved so that the overflow check
-    // covers the whole push
-    std::vector<NormClass> all;
-    for (auto& kv : classes) all.push_back(NormClass{kv.first, &kv.second.per_part, &kv.second.busiest});
-    LaunchNormWorks(all, opt_kind, part_dev);
-  } else {
-    for (auto& kv : classes) LaunchWorks(kv.first, kv.second.per_part, kv.second.busiest, opt_kind, part_dev);
-  }
-
-  // ---- epilogue -------------------------------------------------------------------
-  for (size_t i = 0; i < temps.size(); ++i) {
-    DeviceGuard dg(temp_dev[i]);
-    CUDA_CALL(cudaFreeAsync(temps[i], rt->Dev(temp_dev[i]).stream));
-  }
-  if (!collective) {
-    // destinations on other GPUs were written by the root's kernel
-    for (int dev : touched) if (dev != root_dev) rt->StreamWait(dev, root_dev);
-  }
-  for (KeyState* ks : callback_keys) {
-    Replica* root = FindReplica(*ks, part_dev[mp_mode ? pg->rank() : 0]);
-    RunCallbackUpdater(*ks, *root);
-  }
-  for (auto& pc : post) CopyFromTo(pc.src, pc.dst);
-  for (int dev : touched) rt->ReleaseToUser(dev);
+  IssuePlan(plan);
 
   // ---- remember this call: the second identical call in a row (nothing else touched its keys in between)
   // leaves a plan behind, the third and later ones replay it
-  if (rec_on && !callback && !rec_bad && temps.empty()) {
-    rec.epochs.clear();
-    for (int key : rec.keys) rec.epochs.push_back(keys_.find(key)->second.epoch);
-    rec.cfg_epoch = cfg_epoch_;
-    rec.tuning_epoch = rt->tuning_epoch;
-    rec.recorded = rec_repeat;
-    if (!rec.recorded) { rec.launches.clear(); rec.pre_copies.clear(); rec.post_copies.clear(); }
+  if (rec_on && plan.repeatable && plan.staged.empty() && plan.callback_keys.empty()) {
+    for (int key : plan.keys) plan.epochs.push_back(keys_.find(key)->second.epoch);
+    plan.cfg_epoch = cfg_epoch_;
+    plan.tuning_epoch = Runtime::Get()->tuning_epoch;
+    plan.recorded = rec_repeat;
+    if (!plan.recorded) { plan.launches.clear(); plan.pre_copies.clear(); plan.post_copies.clear(); }
     if (plans_.size() > 256) plans_.clear();          // (a training loop has a handful of distinct calls)
-    plans_[rec_hash] = std::move(rec);
+    plans_[rec_hash] = std::move(plan);
+  }
+}
+
+// ---- replicas and optimizer state, laid out for this call's participants -------------------------------
+void KVStore::KeyReplicas(CallPlan& plan, KeyBuild& k) {
+  Runtime* rt = Runtime::Get();
+  KeyState& ks = k.ks;
+  const std::vector<int>& part_dev = plan.part_dev;
+  const int n_part = static_cast<int>(part_dev.size());
+  const bool callback = updater_ != nullptr && hier_phase_ != 1;
+  k.rep.assign(n_part, nullptr);
+  for (int p = k.first; p <= k.last; ++p) {
+    Touch(&plan.touched, part_dev[p]);
+    EnsureReplica(ks, part_dev[p]);
+  }
+  // EnsureReplica may reallocate ks.reps: resolve pointers afterwards
+  for (int p = k.first; p <= k.last; ++p) k.rep[p] = FindReplica(ks, part_dev[p]);
+
+  const bool lowp = ks.dtype == kFloat16 || ks.dtype == kBfloat16;
+  k.mp = plan.fused && (opt_.multi_precision || lowp);
+  if (plan.fused) {
+    MXKV_CHECK(ks.dtype == kFloat32 || lowp) << "fused optimizers need float32/float16/bfloat16 keys";
+    for (int p = k.first; p <= k.last; ++p) EnsureState(ks, *k.rep[p], k.mp);
+  }
+
+  k.two_shot = plan.collective && !hier_whole_keys_ &&
+               static_cast<int64_t>(ks.size * DTypeSize(ks.dtype)) >= rt->twoshot_bytes &&
+               ks.size >= static_cast<int64_t>(n_part) * 128;
+  if (hier_phase_ != 1 && ks.local_world > 0 &&
+      (callback || !(k.two_shot && ks.local_world == n_part && ks.shard_devs == part_dev))) {
+    GatherLocal(ks);
+    plan.repeatable = false;
+    for (int p = k.first; p <= k.last; ++p) EnsureReplica(ks, part_dev[p]);
+    for (int p = k.first; p <= k.last; ++p) k.rep[p] = FindReplica(ks, part_dev[p]);
+  }
+  if (plan.fused) {
+    // the optimizer state is laid out for this call's shape: sharded over the n participants of a
+    // two-shot push, complete on every replica otherwise (also when a key that used to be sharded is
+    // now pushed from one GPU only)
+    const int want = (plan.collective && k.two_shot) ? n_part : 0;
+    const bool same = ks.state_world == want && (want == 0 || ks.state_devs == part_dev);
+    if (ks.count > 0 && !same) { GatherState(ks); plan.repeatable = false; }
+    ks.state_world = want;
+    if (want > 0) ks.state_devs = part_dev; else ks.state_devs.clear();
+    // a replica that sat out earlier updates (its GPU did not take part) first takes over the state of
+    // one that did; after this call only the participants' state is current
+    for (int p = k.first; p <= k.last; ++p) SyncState(ks, *k.rep[p]);
+    for (auto& r : ks.reps) {
+      bool part = false;
+      for (int p = k.first; p <= k.last; ++p) part = part || (&r == k.rep[p]);
+      if (!part) r.state_fresh = false;
+    }
+  }
+}
+
+// ---- sources as addressable pointers: srcptr[p][k] is the address of source k for the kernel running as
+// participant p.  Values the kernel cannot read where they are get a staging step into the plan.
+std::vector<std::vector<const void*>> KVStore::KeySources(CallPlan& plan, KeyBuild& k) {
+  Runtime* rt = Runtime::Get();
+  ProcessGroup* pg = PG();
+  const Group& g = k.g();
+  const int n_part = static_cast<int>(plan.part_dev.size());
+  const int n_src = static_cast<int>(g.vals.size());
+  const int root_dev = plan.root_dev;
+  std::vector<std::vector<const void*>> srcptr(n_part, std::vector<const void*>(plan.collective ? n_part : n_src));
+  auto stage = [&](const NDArray& v, int dev) -> const void* {   // a temporary on `dev`, filled by IssuePlan
+    void* t = nullptr;
+    DeviceGuard dg(dev);
+    CUDA_CALL(cudaMallocAsync(&t, v.nbytes() ? v.nbytes() : 16, rt->Dev(dev).stream));
+    plan.staged.push_back(StagedValue{v, t, dev});
+    return t;
+  };
+  if (pg != nullptr && hier_phase_ == 2) {
+    srcptr[pg->rank()].assign(1, hier_base_.at(k.ks.key));
+  } else if (pg != nullptr) {
+    const NDArray& v = g.vals[0];
+    if (plan.collective) {
+      NDArray sym_src = v;
+      if (!v.symmetric()) {
+        Replica& r = *k.rep[pg->rank()];
+        if (r.stage.is_none()) r.stage = NDArray::Empty(k.ks.shape, Context{kGPU, pg->dev()}, k.ks.dtype, true);
+        plan.pre_copies.emplace_back(v, r.stage);   // D2D or H2D
+        sym_src = r.stage;
+      }
+      for (int q = 0; q < n_part; ++q) srcptr[pg->rank()][q] = sym_src.peer_data(q);
+    } else {
+      srcptr[pg->rank()][0] = k.devs[0] < 0 ? stage(v, pg->dev()) : v.data();
+    }
+  } else if (plan.collective) {
+    for (int p = 0; p < n_part; ++p)
+      for (int q = 0; q < n_part; ++q) srcptr[p][q] = g.vals[q].data();
+  } else {
+    for (int s = 0; s < n_src; ++s) {
+      const int dev = k.devs[s];
+      const bool direct = dev == root_dev || (dev >= 0 && (rt->EnablePeerAccess({root_dev, dev}),
+                                                           rt->PeerOK(root_dev, dev)));
+      Touch(&plan.touched, dev);
+      if (direct && dev != root_dev) plan.pre_waits.emplace_back(root_dev, dev);   // foreign GPU read by the root kernel
+      // a host value, or no P2P: staged on the root
+      srcptr[0][s] = direct ? g.vals[s].data() : stage(g.vals[s], root_dev);
+    }
+  }
+  return srcptr;
+}
+
+// ---- MXNET_KVSTORE_USETREE: which tree(s) this key's sum goes up ------------------------------------
+// Two values add the same way in any order, and the integer dtypes wrap: only three or more floating-point
+// values are order-sensitive.  Host-resident values and multi-node stores keep the plain order (the
+// reference's tree needs every value on its own GPU, comm_tree.h:108-121).
+void KVStore::KeyTree(const CallPlan& plan, KeyBuild& k) {
+  const KeyState& ks = k.ks;
+  const int n_part = static_cast<int>(plan.part_dev.size());
+  if (!(tree_ && plan.collective && n_part >= 3 && hier_phase_ == 0 &&
+        (ks.dtype == kFloat32 || ks.dtype == kFloat16 || ks.dtype == kBfloat16 || ks.dtype == kFloat64)))
+    return;
+  MXKV_CHECK(!(plan.fused && IsNormOpt(opt_.kind)))
+      << "MXNET_KVSTORE_USETREE=1: the layer-wise optimizers (LAMB / LANS / LARS) are not served in tree order";
+  MXKV_CHECK(TreeKernelAvailable(ks.dtype, plan.fused ? opt_.kind : OPT_NONE, k.mp ? 1 : 0))
+      << "MXNET_KVSTORE_USETREE=1: no tree kernel for dtype " << ks.dtype << " with optimizer kind " << opt_.kind;
+  ProcessGroup* pg = PG();
+  k.tree = &TreePlanFor(pg != nullptr ? pg->rank_devs() : plan.part_dev);
+  const int64_t rows = ks.shape.empty() ? 1 : ks.shape[0];
+  k.tree_sliced = ks.size > tree_bound_ && rows >= 2 * static_cast<int64_t>(n_part);
+}
+
+// ---- destinations: what the kernels write (replicas, the updater's merge buffer, the outputs they can write
+// themselves), the NVLS choice, the copies out of a replica afterwards, and which replicas are fresh after the call
+std::vector<KVStore::Dest> KVStore::KeyDests(CallPlan& plan, KeyBuild& k) {
+  Runtime* rt = Runtime::Get();
+  ProcessGroup* pg = PG();
+  const bool mp_mode = pg != nullptr;
+  const bool callback = updater_ != nullptr && hier_phase_ != 1;
+  const Group& g = k.g();
+  KeyState& ks = k.ks;
+  const std::vector<int>& part_dev = plan.part_dev;
+  const int n_part = static_cast<int>(part_dev.size());
+  const bool collective = plan.collective, two_shot = k.two_shot;
+  const int root_dev = plan.root_dev;
+  std::vector<Dest> dests;
+  auto add_dest_sp = [&](void* ptr, int dev) {
+    Dest d;
+    for (int p = 0; p < kMaxRanks; ++p) d.ptr[p] = ptr;
+    d.owner = -1;
+    for (int p = 0; p < n_part; ++p) if (part_dev[p] == dev) d.owner = p;
+    dests.push_back(d);
+  };
+  if (callback) {
+    Replica& root = *k.rep[k.first];
+    if (root.merged.is_none())
+      root.merged = NDArray::Empty(ks.shape, Context{kGPU, root.dev}, ks.dtype, mp_mode);
+    if (mp_mode && collective) {
+      Dest d; d.owner = -2;   // every rank owns its own copy
+      for (int p = 0; p < n_part; ++p) d.ptr[p] = root.merged.peer_data(p);
+      dests.push_back(d);
+    } else {
+      add_dest_sp(root.merged.data(), root.dev);
+    }
+    plan.callback_keys.push_back(&ks);
+  } else {
+    // which outputs can be written by the kernel itself?
+    std::vector<char> out_direct(g.outs.size(), 0);
+    bool need_post = false;
+    if (k.write_outs) {
+      int budget = kMaxOut - 1 - (mp_mode ? 1 : static_cast<int>(ks.reps.size()));
+      for (size_t oi = 0; oi < g.outs.size(); ++oi) {
+        NDArray* o = g.outs[oi];
+        MXKV_CHECK(o->size() == ks.size && o->dtype() == ks.dtype)
+            << "pushpull: output does not match key " << ks.key;
+        const Context oc = o->ctx();
+        bool direct = false;
+        if (oc.is_gpu() && budget > 0) {
+          if (mp_mode) {
+            direct = collective ? o->symmetric() : (oc.dev_id == pg->dev());
+          } else {
+            for (int p = 0; p < n_part; ++p) if (part_dev[p] == oc.dev_id) direct = true;
+          }
+          // one-shot in-place allreduce: peers still read this buffer while we would write it
+          if (direct && collective && !two_shot) {
+            for (auto& v : g.vals)
+              if (Overlap(o->data(), o->nbytes(), v.data(), v.nbytes())) direct = false;
+          }
+          if (direct && !Aligned16(o->data())) direct = false;
+          if (direct && k.groups.size() > 1 && k.alias.OverlapsOther(o->data(), o->nbytes(), static_cast<int>(k.gi)))
+            direct = false;
+        }
+        out_direct[oi] = direct ? 1 : 0;
+        if (direct) --budget; else need_post = true;
+      }
+    }
+    // Two-shot keys keep the stored value sharded (rank p owns shard p of its own replica) unless
+    // an output has to be copied out of a complete replica afterwards: the all-gather then moves
+    // each shard over NVLink once per peer (into the outputs) instead of twice.
+    // NVLS: every array of the key is bound to a multicast object (and nothing has to be copied
+    // out of a complete replica afterwards)
+    // (auto: above 4 ranks.  Per direction the switch path moves S(1 + 1/n) against 2S(n-1)/n of
+    // the peer path: 1.5x more at n=2, 1.2x less at n=4 -- where the peer path is still kept because
+    // it is bit-exact --, 1.56x less at n=8)
+    if (mp_mode && collective && !hier_ && k.tree == nullptr &&
+        (rt->nvls_mode >= 2 || (rt->nvls_mode == 1 && n_part > 4)) &&
+        !(plan.fused && IsNormOpt(opt_.kind)) && ks.dtype == kFloat32 && ks.size % 4 == 0 &&
+        g.vals[0].mc_data() != nullptr && Aligned16(g.vals[0].mc_data()) && !(two_shot && need_post)) {
+      k.nvls = true;
+      if (k.write_outs)
+        for (size_t oi = 0; oi < g.outs.size(); ++oi)
+          if (out_direct[oi] && g.outs[oi]->mc_data() == nullptr) k.nvls = false;
+    }
+    const bool shard_local = two_shot && !need_post;
+    if (hier_phase_ == 1) {
+      // the node's sum of this rank's range (the whole key when it is not sharded) goes to the staging slice
+      Dest d; d.owner = collective ? -2 : -1; d.own_only = shard_local;
+      for (int p = 0; p < kMaxRanks; ++p) d.ptr[p] = hier_base_.at(ks.key);
+      if (!collective) d.owner = 0;
+      dests.push_back(d);
+    } else if (mp_mode && collective) {
+      Dest d; d.owner = -2; d.own_only = shard_local;
+      for (int p = 0; p < n_part; ++p) d.ptr[p] = k.rep[pg->rank()]->local.peer_data(p);
+      dests.push_back(d);
+    } else {
+      for (auto& r : ks.reps) {
+        const bool reachable = r.dev == root_dev || collective ||
+                               (rt->EnablePeerAccess({root_dev, r.dev}), rt->PeerOK(root_dev, r.dev));
+        bool is_part = false;
+        for (int p = 0; p < n_part; ++p) if (part_dev[p] == r.dev) is_part = true;
+        if (is_part || (reachable && !collective)) {
+          if (!is_part) { Touch(&plan.touched, r.dev); plan.pre_waits.emplace_back(root_dev, r.dev); }
+          add_dest_sp(r.local.data(), r.dev);
+          dests.back().own_only = shard_local;
+          r.fresh = true;
+        } else {
+          r.fresh = false;          // refreshed lazily by EnsureReplica
+        }
+      }
+    }
+    if (hier_phase_ == 1) {
+      // the stored value is not touched in this phase
+    } else if (shard_local) { ks.local_world = n_part; ks.shard_devs = part_dev; }
+    else ks.local_world = 0;
+    if (k.write_outs) {
+      for (size_t oi = 0; oi < g.outs.size(); ++oi) {
+        NDArray* o = g.outs[oi];
+        const Context oc = o->ctx();
+        if (oc.is_gpu()) Touch(&plan.touched, oc.dev_id);
+        if (out_direct[oi]) {
+          if (mp_mode && collective) {
+            Dest d; d.owner = -2;
+            for (int p = 0; p < n_part; ++p) d.ptr[p] = o->peer_data(p);
+            d.mc = o->mc_data();
+            dests.push_back(d);
+          } else {
+            add_dest_sp(o->data(), oc.dev_id);
+          }
+        } else {
+          // copy out of a replica this call has just written: a replica on the output's own GPU only if
+          // that GPU took part (a replica left over from an earlier device set is stale now)
+          Replica* near = oc.is_gpu() ? FindReplica(ks, oc.dev_id) : nullptr;
+          const int sdev = (near != nullptr && near->fresh) ? oc.dev_id : part_dev[k.first];
+          plan.post_copies.emplace_back(FindReplica(ks, sdev)->local, *o);
+        }
+      }
+    }
+  }
+  MXKV_CHECK(static_cast<int>(dests.size()) <= kMaxOut) << "too many destinations for key " << ks.key;
+  return dests;
+}
+
+// ---- work entries: one per local participant (per tree slice with MXNET_KVSTORE_USETREE), in the key's launch
+// class.  One launch (one pair of rendezvous) serves the one-shot and the two-shot keys of a call: the
+// release/acquire flavour of the end barrier covers both.
+void KVStore::KeyWorks(CallPlan& plan, const KeyBuild& k, const std::vector<std::vector<const void*>>& srcptr,
+                       const std::vector<Dest>& dests) {
+  KeyState& ks = k.ks;
+  const int n_part = static_cast<int>(plan.part_dev.size());
+  const bool collective = plan.collective, two_shot = k.two_shot;
+  float lr = 0.f, wd = 0.f;
+  if (plan.fused) {
+    ks.count += 1;                 // Optimizer._update_count
+    lr = KeyLR(ks);
+    wd = KeyWD(ks);
+  }
+  LaunchClassKey ck{collective ? SYNC_WRITE_PEERS : SYNC_NONE, ks.dtype, k.mp ? 1 : 0};
+  ck.nvls = k.nvls ? 1 : 0;
+  ck.tree = k.tree != nullptr ? 1 : 0;
+  auto it = std::lower_bound(plan.launches.begin(), plan.launches.end(), ck,
+                             [](const PlanLaunch& l, const LaunchClassKey& c) { return l.ck < c; });
+  if (it == plan.launches.end() || ck < it->ck)
+    it = plan.launches.insert(it, PlanLaunch{ck, std::vector<std::vector<TensorWork>>(n_part), {},
+                                             std::vector<std::vector<int>>(n_part)});
+  PlanLaunch& l = *it;
+  const int64_t shard = two_shot ? ShardLen(ks.size, n_part) : ks.size;
+  l.busiest.push_back(std::min<int64_t>(ks.size, shard));
+  for (int p = k.first; p <= k.last; ++p) {
+    TensorWork tw = two_shot ? ReplicaWork(ks, *k.rep[p], k.mp, std::min<int64_t>(ks.size, shard * p),
+                                           std::min<int64_t>(ks.size, shard * (p + 1)), lr, wd)
+                             : ReplicaWork(ks, *k.rep[p], k.mp, 0, ks.size, lr, wd);
+    if (k.nvls) {                  // the switch sums the replicas: one multicast "source"
+      tw.n_src = 1;
+      tw.src[0] = k.g().vals[0].mc_data();
+    } else {
+      tw.n_src = static_cast<int>(srcptr[p].size());
+      for (int s = 0; s < tw.n_src; ++s) tw.src[s] = srcptr[p][s];
+    }
+    std::vector<void*> mc_outs;
+    for (auto& d : dests) {
+      if (d.owner == -2) {           // MP: one copy per rank
+        if (two_shot && !d.own_only) {
+          if (k.nvls) { mc_outs.push_back(d.mc); continue; }
+          for (int q = 0; q < n_part; ++q) tw.out[tw.n_out++] = d.ptr[q];
+        } else {
+          tw.out[tw.n_out++] = d.ptr[p];
+        }
+        continue;
+      }
+      const bool mine = !collective || (two_shot && !d.own_only) || d.owner == p || (d.owner == -1 && p == 0);
+      if (mine) tw.out[tw.n_out++] = d.ptr[p];
+    }
+    for (void* m : mc_outs) { tw.out[tw.n_out++] = m; tw.n_mc++; }
+    MXKV_CHECK(tw.n_out <= kMaxOut) << "too many destinations for key " << ks.key;
+    tw.flags = WorkFlags(tw, DTypeSize(ks.dtype) == 4 && ks.size % 4 == 0);
+    if (k.nvls) MXKV_CHECK(tw.flags & kWorkVec16) << "NVLS arrays must be 16-byte aligned";
+    if (k.tree != nullptr) AppendTreeWorks(tw, *k.tree, k.tree_sliced, ks, n_part, &l.per_part[p]);
+    else l.per_part[p].push_back(tw);
+    l.key_idx[p].resize(l.per_part[p].size(), static_cast<int>(k.gi));
   }
 }
 
@@ -2155,7 +2128,7 @@ void KVStore::LaunchWorks(const LaunchClassKey& ck, std::vector<std::vector<Tens
     bool ok = true;
     int max_src = 1;
     for (int p = my_first; p <= my_last; ++p)
-      for (auto& t : per_part[p]) { ok = ok && (t.pad_ & 2); max_src = std::max(max_src, t.n_src); }
+      for (auto& t : per_part[p]) { ok = ok && (t.flags & kWorkStaged); max_src = std::max(max_src, t.n_src); }
     const int extra = (opt_kind != OPT_NONE ? 1 : 0) +
                       ((opt_kind == OPT_SGD_MOM || opt_kind == OPT_ADAM || opt_kind == OPT_ADAMW) ? 1 : 0) +
                       ((opt_kind == OPT_ADAM || opt_kind == OPT_ADAMW) ? 1 : 0);
@@ -2251,6 +2224,19 @@ void KVStore::LaunchWorks(const LaunchClassKey& ck, std::vector<std::vector<Tens
   }
 }
 
+TensorWork KVStore::ReplicaWork(const KeyState& ks, const Replica& r, bool mp, int64_t begin, int64_t end, float lr,
+                                float wd) const {
+  TensorWork tw;
+  std::memset(&tw, 0, sizeof(tw));
+  tw.w = r.local.data();
+  tw.w32 = mp ? static_cast<float*>(r.w32.data()) : nullptr;
+  tw.s0 = r.s0.is_none() ? nullptr : static_cast<float*>(r.s0.data());
+  tw.s1 = r.s1.is_none() ? nullptr : static_cast<float*>(r.s1.data());
+  tw.begin = begin; tw.end = end;
+  tw.lr = lr; tw.wd = wd; tw.eta = KeyEta(ks); tw.key = ks.key;
+  return tw;
+}
+
 // A launch that involves one GPU only (no rendezvous), whatever the deployment shape.
 void KVStore::LaunchLocal(const LaunchClassKey& ck, const TensorWork& tw, int opt_kind, int dev) {
   ProcessGroup* pg = PG();
@@ -2295,7 +2281,7 @@ void KVStore::GatherLocal(KeyState& ks) {
     }
     tw.begin = std::min<int64_t>(ks.size, shard * p);
     tw.end = std::min<int64_t>(ks.size, shard * (p + 1));
-    tw.pad_ = 1 | ((ks.dtype == kFloat32 && ks.size % 4 == 0) ? 2 : 0);
+    tw.flags = WorkFlags(tw, ks.dtype == kFloat32 && ks.size % 4 == 0);
     per_part[p].push_back(tw);
   }
   LaunchClassKey ck{SYNC_WRITE_PEERS, ks.dtype, 0};

@@ -192,9 +192,22 @@ class KVStore {
     std::vector<NDArray> vals;         // pushed values (dense)
     std::vector<NDArray*> outs;        // pull destinations (may be empty)
   };
-  // the fused reduce(+update)(+broadcast) over a list of dense key groups
+  // the fused reduce(+update)(+broadcast) over a list of dense key groups: builds the call's CallPlan key by key
+  // (the stages below, none of which launches or touches a caller array), then IssuePlan
   void ReduceUpdate(std::vector<Group>& groups, bool write_outs);
   void PlaceKey(const Group& g, KeyState& ks, std::vector<int>* devs, std::vector<int>* key_part, bool* key_collective);
+  struct CallPlan;
+  struct KeyBuild;                     // one key of the call being built (kvstore.cc)
+  struct Dest;
+  void KeyReplicas(CallPlan& p, KeyBuild& k);
+  std::vector<std::vector<const void*>> KeySources(CallPlan& p, KeyBuild& k);
+  void KeyTree(const CallPlan& p, KeyBuild& k);
+  std::vector<Dest> KeyDests(CallPlan& p, KeyBuild& k);
+  void KeyWorks(CallPlan& p, const KeyBuild& k, const std::vector<std::vector<const void*>>& srcptr,
+                const std::vector<Dest>& dests);
+  // an entry that updates replica r of ks over [begin, end) (weight, fp32 master, optimizer state, key scalars);
+  // sources, destinations and flags are the caller's
+  TensorWork ReplicaWork(const KeyState& ks, const Replica& r, bool mp, int64_t begin, int64_t end, float lr, float wd) const;
   // busiest[i]: number of elements the busiest rank processes for entry i (fixes the common grid)
   void LaunchWorks(const LaunchClassKey& ck, std::vector<std::vector<TensorWork>>& per_part,
                    const std::vector<int64_t>& busiest, int opt_kind, const std::vector<int>& part_dev);
@@ -255,13 +268,15 @@ class KVStore {
     std::vector<int64_t> busiest;
     std::vector<std::vector<int>> key_idx;     // per entry of per_part: index of its key in CallPlan::keys
   };
+  // What one dense call issues (IssuePlan).  ReduceUpdate builds it; a repeated call keeps it (plans_).
+  struct StagedValue { NDArray src; void* tmp; int dev; };   // a value copied into a cudaMallocAsync temporary
   struct CallPlan {
     std::vector<uint64_t> sig;                 // keys, array addresses / sizes / devices, flags
     std::vector<int> keys;                     // group order
     std::vector<uint64_t> epochs;              // KeyState::epoch of `keys` right after the recorded call
-    std::vector<PlanLaunch> launches;
-    std::vector<int> part_dev;
-    std::vector<int> touched;                  // devices acquired from / released to the framework stream
+    std::vector<PlanLaunch> launches;          // sorted by class key: the launch order of every rank
+    std::vector<int> part_dev;                 // device of participant p (SP) / own device at index rank (MP)
+    std::vector<int> touched;                  // (sorted) devices acquired from / released to the framework stream
     std::vector<std::pair<int, int>> pre_waits;                 // StreamWait(waiter, signaler) before the launches
     std::vector<std::pair<NDArray, NDArray>> pre_copies;        // staging copies (src, dst) before the launches
     std::vector<std::pair<NDArray, NDArray>> post_copies;       // outputs copied out of a replica afterwards
@@ -270,7 +285,13 @@ class KVStore {
     int root_dev = -1;
     uint64_t cfg_epoch = 0, tuning_epoch = 0;
     bool recorded = false;                     // false: only `sig` / `epochs` of the last identical slow call
+    // per-call work a replay never repeats; a plan that has any is not kept
+    std::vector<StagedValue> staged;           // host values / values without P2P, freed after the launches
+    std::vector<KeyState*> callback_keys;      // keys whose Python updater runs after the launches
+    bool repeatable = true;                    // false: the build gathered a sharded value or optimizer state
   };
+  void IssuePlan(CallPlan& p);
+  bool SamePlan(const CallPlan& a, const CallPlan& b) const;
   // The signature is taken from the call's raw arguments (TryReplayRaw, below) so that a hit costs no grouping,
   // no NDArray copies and no allocation; ReduceUpdate records under it when the call reached it as ONE fused
   // reduce over all of its keys (raw_single_).
@@ -279,7 +300,6 @@ class KVStore {
   bool raw_pending_ = false, raw_single_ = false;
   bool PlanEpochsMatch(const CallPlan& p) const;
   void PlanPatch(CallPlan& p, bool commit_counts);
-  void PlanReplay(CallPlan& p);
   struct Deferred {
     int kind;                               // 0 push, 1 pushpull
     std::vector<int> vkeys, okeys;

@@ -79,7 +79,7 @@ void KVStore::LaunchNormWorks(std::vector<NormClass>& classes, int opt_kind, con
       std::vector<NormWork> nw(w.size());
       for (size_t i = 0; i < w.size(); ++i) {
         const TensorWork& t = w[i];
-        KeyState& ks = GetKey(t.reserved_);
+        KeyState& ks = GetKey(t.key);
         Replica* r = FindReplica(ks, dev);
         MXKV_CHECK(r != nullptr && !r->aux0.is_none() && !r->nrm.is_none())
             << "key " << ks.key << ": optimizer scratch missing";
@@ -100,7 +100,7 @@ void KVStore::LaunchNormWorks(std::vector<NormClass>& classes, int opt_kind, con
         n.c1 = 1.0f - std::pow(static_cast<float>(opt_.beta1), tcount);
         n.c2 = 1.0f - std::pow(static_cast<float>(opt_.beta2), tcount);
         n.n_src = t.n_src; n.n_out = t.n_out;
-        n.flags = (t.pad_ & 1) | (opt_.no_trust.count(ks.key) ? 2 : 0);
+        n.flags = (t.flags & kWorkVec16) | (opt_.no_trust.count(ks.key) ? 2 : 0);
         // a sharded (two-shot) key: every rank holds the sums of its shard only
         const bool sharded = collective && (t.end - t.begin) != ks.size;
         if (sharded) {
@@ -227,7 +227,7 @@ void KVStore::LaunchNormWorks(std::vector<NormClass>& classes, int opt_kind, con
   }
   if (opt_.skip_nonfinite) {
     for (auto& cls : classes)
-      for (auto& t : (*cls.per_part)[my_first]) last_norm_keys_.push_back(t.reserved_);
+      for (auto& t : (*cls.per_part)[my_first]) last_norm_keys_.push_back(t.key);
   }
 }
 

@@ -363,15 +363,10 @@ void KVStore::PushRowSparse(KeyState& ks, const std::vector<NDArray>& vals) {
       CUDA_CALL(cudaMemsetAsync(gd, 0, static_cast<size_t>(ks.size) * 4, s));
       CheckLaunch(LaunchRspScatter(gd, r.rsp_merged.idx_ptr(), r.rsp_merged.d_nnz(), r.rsp_merged.cap_rows(), L,
                                    static_cast<const float*>(r.rsp_merged.data()), s), "rsp_scatter");
-      TensorWork tw;
-      std::memset(&tw, 0, sizeof(tw));
+      TensorWork tw = ReplicaWork(ks, r, false, 0, ks.size, lr, wd);
       tw.src[0] = gd; tw.n_src = 1;
       tw.out[0] = r.local.data(); tw.n_out = 1;
-      tw.w = r.local.data();
-      tw.s0 = A.s0; tw.s1 = A.s1;
-      tw.begin = 0; tw.end = ks.size;
-      tw.lr = lr; tw.wd = wd; tw.eta = KeyEta(ks); tw.reserved_ = ks.key;
-      tw.pad_ = (ks.size % 4 == 0 && Aligned16(r.local.data())) ? 1 : 0;
+      tw.flags = ks.size % 4 == 0 ? WorkFlags(tw, false) : 0;   // (tables of other sizes keep the scalar path)
       const int kind = opt_.kind == OPT_SGD ? OPT_SGD_STD : (opt_.kind == OPT_ADAM ? OPT_ADAM_STD : opt_.kind);
       LaunchLocal(LaunchClassKey{SYNC_NONE, kFloat32, 0}, tw, kind, dev);
       CUDA_CALL(cudaFreeAsync(gd, s));
@@ -593,15 +588,10 @@ void KVStore::HierPushRowSparse(KeyState& ks, const std::vector<NDArray>& vals) 
     CUDA_CALL(cudaMemsetAsync(gd, 0, static_cast<size_t>(ks.size) * 4, s));
     CheckLaunch(LaunchRspScatter(gd, r.rsp_merged.idx_ptr(), r.rsp_merged.d_nnz(), r.rsp_merged.cap_rows(), L,
                                  static_cast<const float*>(r.rsp_merged.data()), s), "rsp_scatter");
-    TensorWork tw;
-    std::memset(&tw, 0, sizeof(tw));
+    TensorWork tw = ReplicaWork(ks, r, false, 0, ks.size, lr, wd);
     tw.src[0] = gd; tw.n_src = 1;
     tw.out[0] = r.local.data(); tw.n_out = 1;
-    tw.w = r.local.data();
-    tw.s0 = B.s0; tw.s1 = B.s1;
-    tw.begin = 0; tw.end = ks.size;
-    tw.lr = lr; tw.wd = wd; tw.eta = KeyEta(ks); tw.reserved_ = ks.key;
-    tw.pad_ = (ks.size % 4 == 0 && Aligned16(r.local.data())) ? 1 : 0;
+    tw.flags = ks.size % 4 == 0 ? WorkFlags(tw, false) : 0;   // (tables of other sizes keep the scalar path)
     const int kind = opt_.kind == OPT_SGD ? OPT_SGD_STD : (opt_.kind == OPT_ADAM ? OPT_ADAM_STD : opt_.kind);
     LaunchLocal(LaunchClassKey{SYNC_NONE, kFloat32, 0}, tw, kind, dev);
     CUDA_CALL(cudaFreeAsync(gd, s));

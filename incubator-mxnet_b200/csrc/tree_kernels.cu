@@ -128,7 +128,7 @@ kv_dense_tree_kernel(DenseLaunch L) {
     const int64_t cb = tw.begin + (c - L.chunk_prefix[lo]) * L.chunk_elems;
     const int64_t ce = (cb + L.chunk_elems < tw.end) ? cb + L.chunk_elems : tw.end;
     int64_t scalar_from = cb;
-    if (tw.pad_ & 1) {  // every pointer 16-byte aligned and begin % 8 == 0
+    if (tw.flags & kWorkVec16) {  // every pointer 16-byte aligned and begin % 8 == 0
       const int64_t nvec = (ce - cb) / NV;
       for (int64_t v = threadIdx.x; v < nvec; v += blockDim.x)
         tree_packet<T, OPT, MP, NV>(tw, cb + v * NV, h, native_half_add);

@@ -679,6 +679,35 @@ def test_sharding_threshold_and_chunking_change_between_calls():
         check_call(_LIB.MXKVB200SetTuning(ctypes.c_int64(8192), 512, 0, -1))
 
 
+def test_empty_trailing_shard_keeps_the_staged_kernel():
+    """A two-shot float32 key of 516 elements over 4 GPUs: shards of 256, so the last rank's range is empty and
+    starts at 516, which is not on a packet boundary.  An empty range reads and writes nothing, so it must not take
+    the launch class (here with a larger key) off the staged kernel -- in one-process-per-GPU mode every rank
+    decides the variant from its own entries, and the ranks would disagree on the grid."""
+    _need(4)
+    import ctypes
+    from mxnet_b200.base import _LIB, check_call
+    devs = list(range(4))
+    sizes = [516, 70000]
+    rng = _rng(21)
+    try:
+        check_call(_LIB.MXKVB200SetTwoShotBytes(ctypes.c_int64(1024)))
+        kv = mx.kv.create("device")
+        kv.init([0, 1], [mx.nd.zeros((E,), mx.gpu(0)) for E in sizes])
+        vals = [[rng.uniform(-1, 1, E).astype(np.float32) for _ in devs] for E in sizes]
+        outs = [[mx.nd.empty((E,), mx.gpu(d)) for d in devs] for E in sizes]
+        bulk0, thread0 = mx.kv.launch_count("bulk"), mx.kv.launch_count("per_thread")
+        kv.pushpull([0, 1], [[mx.nd.array(v, mx.gpu(d)) for v, d in zip(vs, devs)] for vs in vals], out=outs)
+        assert mx.kv.launch_count("per_thread") == thread0
+        assert mx.kv.launch_count("bulk") - bulk0 == len(devs)
+        for vs, os_ in zip(vals, outs):
+            want = O.sum_device(vs)
+            for o in os_:
+                assert _bits_equal(o.asnumpy(), want)
+    finally:
+        check_call(_LIB.MXKVB200SetTwoShotBytes(ctypes.c_int64(262144)))
+
+
 @pytest.mark.parametrize("seed", list(range(12 + _EXTRA)))
 def test_randomized_dense_keys_with_row_sparse_gradients(seed):
     """Dense weights updated on the store by a random mix of dense and row_sparse gradients (Parameter(grad_stype=
