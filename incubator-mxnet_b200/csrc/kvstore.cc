@@ -1244,13 +1244,9 @@ void KVStore::ReduceUpdateCompressed(std::vector<Group>& groups, bool write_outs
       for (auto& r : ks.reps) if (std::find(consumers.begin(), consumers.end(), r.dev) == consumers.end()) consumers.push_back(r.dev);
       rt->EnablePeerAccess(consumers);
     }
-    SyncArgs sync;
-    std::memset(&sync, 0, sizeof(sync));
+    SyncArgs sync{};
     if (world > 1) {
-      sync.self = rt->Dev(pg->dev()).signal_pad;
-      for (int q = 0; q < world; ++q) sync.peers[q] = pg->signal_pad(q);
-      sync.world = world; sync.rank = pg->rank(); sync.mode = SYNC_WRITE_PEERS;
-      sync.timeout = rt->spin_timeout_cycles;
+      sync = GroupSync(SYNC_WRITE_PEERS);
       DeviceGuard dg(pg->dev());
       sync.epoch = rt->NextSyncEpoch(pg);
       MXKV_CHECK(LaunchBarrier(sync, rt->Dev(pg->dev()).stream) == 0) << "barrier launch failed";   // codes published
@@ -1382,7 +1378,7 @@ void KVStore::HierReduceUpdate(std::vector<Group>& groups, bool write_outs) {
       KeyState& ks = GetKey(g.key);
       Replica& root = *FindReplica(ks, dev);
       InterNodeSum(root.merged.data(), ks.size, ks.dtype, dev);
-      RunCallbackUpdater(ks, root);
+      RunCallbackUpdater(ks, root, root.merged);
       ks.local_world = 0;
     }
     rt->ReleaseToUser(dev);
@@ -1547,7 +1543,10 @@ void KVStore::IssuePlan(CallPlan& p) {
     for (int dev : p.touched) if (dev != p.root_dev) rt->StreamWait(dev, p.root_dev);
   if (!p.callback_keys.empty()) {
     ProcessGroup* pg = PG();
-    for (KeyState* ks : p.callback_keys) RunCallbackUpdater(*ks, *FindReplica(*ks, p.part_dev[pg ? pg->rank() : 0]));
+    for (KeyState* ks : p.callback_keys) {
+      Replica& root = *FindReplica(*ks, p.part_dev[pg ? pg->rank() : 0]);
+      RunCallbackUpdater(*ks, root, root.merged);
+    }
   }
   for (auto& c : p.post_copies) CopyFromTo(c.first, c.second);
   for (int dev : p.touched) rt->ReleaseToUser(dev);
@@ -2294,14 +2293,36 @@ void KVStore::GatherLocal(KeyState& ks) {
   }
 }
 
+SyncArgs KVStore::GroupSync(int mode) const {
+  Runtime* rt = Runtime::Get();
+  ProcessGroup* pg = PG();
+  SyncArgs sync;
+  std::memset(&sync, 0, sizeof(sync));
+  sync.self = rt->Dev(pg->dev()).signal_pad;
+  for (int q = 0; q < pg->world(); ++q) sync.peers[q] = pg->signal_pad(q);
+  sync.world = pg->world(); sync.rank = pg->rank(); sync.mode = mode;
+  sync.timeout = rt->spin_timeout_cycles;
+  return sync;
+}
+
+SyncArgs KVStore::LocalSync(int dev) {
+  Runtime* rt = Runtime::Get();
+  SyncArgs sync;
+  std::memset(&sync, 0, sizeof(sync));
+  sync.self = rt->Dev(dev).signal_pad;
+  sync.world = 1; sync.rank = 0; sync.mode = SYNC_NONE;
+  sync.timeout = rt->spin_timeout_cycles;
+  return sync;
+}
+
 // updater_(key, merged, &local) on the caller thread (kvstore_local.h:259-277); the callee owns and
 // frees both handles (c_api.cc:3066-3080).  The embedding framework computes on its own stream:
 // fence it on the reduce, then make the engine stream wait for whatever the callback enqueued.
-void KVStore::RunCallbackUpdater(KeyState& ks, Replica& root) {
+void KVStore::RunCallbackUpdater(KeyState& ks, Replica& root, const NDArray& merged) {
   Runtime* rt = Runtime::Get();
   rt->Dev(root.dev).engine_dirty = true;
   rt->Fence(root.dev);
-  NDHandle* recv = new NDHandle(root.merged);
+  NDHandle* recv = new NDHandle(merged);
   NDHandle* local = new NDHandle(root.local);
   if (key_type_ == kStringKey && str_updater_ != nullptr) {
     const std::string& sk = reverse_str_key_dict_[ks.key];

@@ -21,6 +21,7 @@
 #include <unordered_map>
 #include <unordered_set>
 #include "ndarray.h"
+#include "rsp_kernels.h"
 #include "topology.h"
 
 namespace mxkv {
@@ -222,8 +223,20 @@ class KVStore {
   void GatherLocal(KeyState& ks);
   bool HostPipelined(std::vector<Group>& groups, bool write_outs);
   void ReduceUpdateCompressed(std::vector<Group>& groups, bool write_outs);
-  void RunCallbackUpdater(KeyState& ks, Replica& root);
+  // the Python updater on (merged, root's stored value)
+  void RunCallbackUpdater(KeyState& ks, Replica& root, const NDArray& merged);
+  // rendezvous arguments (epoch left 0): the process group's ranks in `mode`, or one GPU alone (SYNC_NONE: the grid
+  // barrier of the fused row_sparse kernels)
+  SyncArgs GroupSync(int mode) const;
+  static SyncArgs LocalSync(int dev);
+  // row_sparse push (kvstore_rsp.cc): the single-node and the multi-node form share the stages below
   void PushRowSparse(KeyState& ks, const std::vector<NDArray>& vals);
+  void RowSparseKeyFor(KeyState& ks);
+  bool RowSparseFused() const;
+  RspSources PublishRowSparse(const KeyState& ks, Replica& r, const NDArray& v, bool fill);
+  RspRowArgs RowArgs(const KeyState& ks, const Replica& r, const RspSources& S, bool merge, bool update, bool assign,
+                     float lr, float wd) const;
+  void MergeRows(KeyState& ks, Replica& r, const RspSources& S, int64_t cap, bool update, bool assign, float lr, float wd);
   void InitRowSparseKey(KeyState& ks, const NDArray& v);
   void PullDenseFromRowSparse(KeyState& ks, const std::vector<NDArray*>& outs);
   void BroadcastFromRank0(KeyState& ks, Replica& r);

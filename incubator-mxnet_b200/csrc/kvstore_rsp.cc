@@ -100,33 +100,181 @@ static void EnsureRspWorkspace(KeyState& ks, Replica& r, int n, int64_t cap) {
   r.rsp_cap = cap;
 }
 
+// source k of the row kernels on GPU dev: the value in place where dev can read it (after its own GPU's stream), else
+// -- host-resident, or on a GPU without peer access -- staged on dev in cudaMallocAsync temporaries (ids, rows, device
+// row count) that the caller frees after the launches
+static void SourceOn(RspSources& S, int k, const NDArray& v, int64_t L, int dev, std::vector<void*>& temps) {
+  Runtime* rt = Runtime::Get();
+  const Context c = v.ctx();
+  if (c.is_gpu() && (c.dev_id == dev || rt->PeerOK(dev, c.dev_id))) {
+    if (c.dev_id != dev) rt->StreamWait(dev, c.dev_id);
+    S.idx[k] = v.idx_ptr();
+    S.val[k] = static_cast<const float*>(v.data());
+    S.nnz[k] = v.d_nnz();
+    return;
+  }
+  cudaStream_t s = rt->Dev(dev).stream;
+  const int64_t nnz = v.nnz();
+  void* ti = nullptr; void* tv = nullptr; int64_t* tn = nullptr;
+  CUDA_CALL(cudaMallocAsync(&ti, std::max<int64_t>(nnz, 1) * 8, s));
+  CUDA_CALL(cudaMallocAsync(&tv, std::max<int64_t>(nnz * L, 1) * 4, s));
+  CUDA_CALL(cudaMallocAsync(reinterpret_cast<void**>(&tn), 16, s));
+  if (nnz > 0) {
+    CopyBytes(v.idx_ptr(), c, ti, Context{kGPU, dev}, nnz * 8);
+    CopyBytes(v.data(), c, tv, Context{kGPU, dev}, nnz * L * 4);
+  }
+  CheckLaunch(LaunchSetI64(tn, nnz, s), "set_nnz");
+  temps.push_back(ti); temps.push_back(tv); temps.push_back(tn);
+  S.idx[k] = static_cast<const int64_t*>(ti);
+  S.val[k] = static_cast<const float*>(tv);
+  S.nnz[k] = tn;
+}
+
+// a key initialised dense that receives row_sparse values
+void KVStore::RowSparseKeyFor(KeyState& ks) {
+  if (ks.stype == kRowSparseStorage) return;
+  MXKV_CHECK(ks.dtype == kFloat32 && !ks.shape.empty()) << "row_sparse values need a float32 key (key " << ks.key << ")";
+  if (ks.local_world > 0) GatherLocal(ks);
+  if (updater_ == nullptr && !opt_.enabled) {
+    // Without an updater the stored value simply becomes the merged value, storage type included
+    // (`local = merged.Copy(...)` on a storage-type mismatch, kvstore_local.h:268-276; the reference's
+    // test_aggregator pushes row_sparse values to keys initialised dense).  The stored value is a
+    // dense-backed table either way, so the key only changes its label.
+    ks.stype = kRowSparseStorage;
+    return;
+  }
+  // Dense weight, row_sparse gradient (gluon Parameter(grad_stype='row_sparse') updated on the store,
+  // trainer.py:204-236; SGDUpdateDnsRspImpl / AdamLazyUpdate..., optimizer_op-inl.h:471-555,1305-1516):
+  // the updater sees (merged row_sparse, stored dense) and the key stays dense.  The rows are updated
+  // on every replica, each with its own complete optimizer state.
+  if (opt_.enabled && updater_ == nullptr && ks.state_world > 0) {
+    GatherState(ks);
+    ks.state_world = 0;
+    ks.state_devs.clear();
+  }
+}
+
+// true: the store's optimizer updates the rows (no Python updater)
+bool KVStore::RowSparseFused() const {
+  const bool fused = opt_.enabled && updater_ == nullptr;
+  if (fused)
+    MXKV_CHECK(opt_.kind == OPT_SGD || opt_.kind == OPT_SGD_MOM || opt_.kind == OPT_ADAM)
+        << "row_sparse gradients: only the lazy SGD / SGD-momentum / Adam updates are fused";
+  return fused;
+}
+
+// One process per GPU: this rank's gradient v goes to r's symmetric staging area (allocated on first use), where every
+// rank reads it; returns every rank's staging area as the sources.  Peers may still be reading the area of the previous
+// push, so a barrier comes first unless that push ended with one (the fused kernel's: rsp_stage_guarded).  `fill`:
+// copy v in and publish its row count behind a second barrier; otherwise the fused kernel does both.
+RspSources KVStore::PublishRowSparse(const KeyState& ks, Replica& r, const NDArray& v, bool fill) {
+  Runtime* rt = Runtime::Get();
+  ProcessGroup* pg = PG();
+  const int64_t L = ks.size / ks.shape[0];
+  const int64_t stage_rows = std::min<int64_t>(ks.shape[0], EnvInt("MXKV_B200_RSP_STAGE_ROWS", 131072));
+  if (r.stage_idx.is_none()) {
+    const Context ctx{kGPU, r.dev};
+    r.stage_idx = NDArray::Empty({stage_rows}, ctx, kInt64, true);
+    r.stage_val = NDArray::Empty({stage_rows * L}, ctx, kFloat32, true);
+    r.stage_nnz = NDArray::Empty({2}, ctx, kInt64, true);
+  }
+  MXKV_CHECK(v.nnz() <= r.stage_idx.size())
+      << "row_sparse gradient with " << v.nnz() << " rows exceeds the staging capacity of "
+      << r.stage_idx.size() << " rows; raise MXKV_B200_RSP_STAGE_ROWS";
+  DeviceGuard g(r.dev);
+  cudaStream_t s = rt->Dev(r.dev).stream;
+  SyncArgs sync = GroupSync(SYNC_WRITE_PEERS);
+  sync.epoch = rt->NextSyncEpoch(pg);
+  if (fill || !r.rsp_stage_guarded) CheckLaunch(LaunchBarrier(sync, s), "barrier");
+  if (fill) {
+    if (v.nnz() > 0) {
+      CopyBytes(v.idx_ptr(), v.ctx(), r.stage_idx.data(), r.stage_idx.ctx(), v.nnz() * 8);
+      CopyBytes(v.data(), v.ctx(), r.stage_val.data(), r.stage_val.ctx(), v.nnz() * L * 4);
+    }
+    CheckLaunch(LaunchSetI64(static_cast<int64_t*>(r.stage_nnz.data()), v.nnz(), s), "set_nnz");
+    sync.epoch = rt->NextSyncEpoch(pg);
+    CheckLaunch(LaunchBarrier(sync, s), "barrier");
+  }
+  r.rsp_stage_guarded = !fill;      // the fused kernel ends with a cross-GPU barrier
+  RspSources S;
+  std::memset(&S, 0, sizeof(S));
+  S.n = pg->world();
+  for (int q = 0; q < S.n; ++q) {
+    S.idx[q] = static_cast<const int64_t*>(r.stage_idx.peer_data(q));
+    S.val[q] = static_cast<const float*>(r.stage_val.peer_data(q));
+    S.nnz[q] = static_cast<const int64_t*>(r.stage_nnz.peer_data(q));
+  }
+  return S;
+}
+
+// The row kernels' arguments on replica r over sources S.  `merge`: the union (and, unless the rows are updated lazily,
+// the summed rows) goes to r's merge workspace.  `update`: the store's optimizer with r's state -- lazily on the touched
+// rows (lazy_update), else afterwards over the whole table (MergeRows).  `assign`: the merged rows replace the table.
+RspRowArgs KVStore::RowArgs(const KeyState& ks, const Replica& r, const RspSources& S, bool merge, bool update,
+                            bool assign, float lr, float wd) const {
+  const bool lazy = update && opt_.lazy_update;
+  RspRowArgs A;
+  std::memset(&A, 0, sizeof(A));
+  if (merge) {
+    A.out_idx = r.rsp_merged.idx_ptr();
+    A.out_val = lazy ? nullptr : static_cast<float*>(r.rsp_merged.data());
+    A.d_nnz_out = r.rsp_merged.d_nnz();
+  }
+  A.table = static_cast<float*>(r.local.data());
+  A.row_len = ks.size / ks.shape[0];
+  A.opt = lazy ? opt_.kind : OPT_NONE;
+  A.assign = assign ? 1 : 0;
+  A.lr = lr; A.wd = wd; A.rescale = opt_.rescale; A.clip = opt_.clip; A.momentum = opt_.momentum;
+  A.beta1 = static_cast<float>(opt_.beta1); A.beta2 = static_cast<float>(opt_.beta2); A.eps = opt_.eps;
+  if (update) {
+    A.s0 = r.s0.is_none() ? nullptr : static_cast<float*>(r.s0.data());
+    A.s1 = r.s1.is_none() ? nullptr : static_cast<float*>(r.s1.data());
+  }
+  bool vec = (A.row_len % 4 == 0) && Aligned16(A.table) && (A.out_val == nullptr || Aligned16(A.out_val)) &&
+             (A.s0 == nullptr || Aligned16(A.s0)) && (A.s1 == nullptr || Aligned16(A.s1));
+  for (int k = 0; k < S.n; ++k) vec = vec && Aligned16(S.val[k]);
+  A.vec = vec ? 1 : 0;
+  return A;
+}
+
+// The union + gather-sum kernels over sources S (up to `cap` rows each) on replica r, into its merge workspace, with
+// RowArgs' update / assignment; an update without lazy_update then runs the reference's standard update.
+void KVStore::MergeRows(KeyState& ks, Replica& r, const RspSources& S, int64_t cap, bool update, bool assign, float lr,
+                        float wd) {
+  Runtime* rt = Runtime::Get();
+  cudaStream_t s = rt->Dev(r.dev).stream;
+  EnsureRspWorkspace(ks, r, S.n, cap);
+  const RspRowArgs A = RowArgs(ks, r, S, true, update, assign, lr, wd);
+  // push without updater: local = merged (kvstore_local.h:279-284) -- rows outside the union vanish
+  if (assign) CUDA_CALL(cudaMemsetAsync(r.local.data(), 0, r.local.nbytes(), s));
+  CheckLaunch(LaunchRspSum(S, A, static_cast<int32_t*>(r.rsp_first.data()), static_cast<int32_t*>(r.rsp_pf.data()),
+                           r.rsp_cap, s), "rsp_sum");
+  rt->launches += 3;
+  r.rsp_merged.set_nnz_device();
+  if (update && !opt_.lazy_update) {
+    // densify the merged gradient (absent rows = 0) and run the dense kernel with the reference's
+    // "Std" arithmetic over the whole table: O(table), as in the reference
+    float* gd = nullptr;
+    CUDA_CALL(cudaMallocAsync(reinterpret_cast<void**>(&gd), static_cast<size_t>(ks.size) * 4, s));
+    CUDA_CALL(cudaMemsetAsync(gd, 0, static_cast<size_t>(ks.size) * 4, s));
+    CheckLaunch(LaunchRspScatter(gd, r.rsp_merged.idx_ptr(), r.rsp_merged.d_nnz(), r.rsp_merged.cap_rows(), A.row_len,
+                                 static_cast<const float*>(r.rsp_merged.data()), s), "rsp_scatter");
+    TensorWork tw = ReplicaWork(ks, r, false, 0, ks.size, lr, wd);
+    tw.src[0] = gd; tw.n_src = 1;
+    tw.out[0] = r.local.data(); tw.n_out = 1;
+    tw.flags = ks.size % 4 == 0 ? WorkFlags(tw, false) : 0;   // (tables of other sizes keep the scalar path)
+    const int kind = opt_.kind == OPT_SGD ? OPT_SGD_STD : (opt_.kind == OPT_ADAM ? OPT_ADAM_STD : opt_.kind);
+    LaunchLocal(LaunchClassKey{SYNC_NONE, kFloat32, 0}, tw, kind, r.dev);
+    CUDA_CALL(cudaFreeAsync(gd, s));
+  }
+}
+
 void KVStore::PushRowSparse(KeyState& ks, const std::vector<NDArray>& vals) {
   if (hier_) { HierPushRowSparse(ks, vals); return; }
   Runtime* rt = Runtime::Get();
   ProcessGroup* pg = PG();
   const bool mp_mode = pg != nullptr;
-  if (ks.stype != kRowSparseStorage) {
-    MXKV_CHECK(ks.dtype == kFloat32 && !ks.shape.empty())
-        << "row_sparse values need a float32 key (key " << ks.key << ")";
-    if (ks.local_world > 0) GatherLocal(ks);
-    if (updater_ == nullptr && !opt_.enabled) {
-      // Without an updater the stored value simply becomes the merged value, storage type included
-      // (`local = merged.Copy(...)` on a storage-type mismatch, kvstore_local.h:268-276; the reference's
-      // test_aggregator pushes row_sparse values to keys initialised dense).  The stored value is a
-      // dense-backed table either way, so the key only changes its label.
-      ks.stype = kRowSparseStorage;
-    } else {
-      // Dense weight, row_sparse gradient (gluon Parameter(grad_stype='row_sparse') updated on the store,
-      // trainer.py:204-236; SGDUpdateDnsRspImpl / AdamLazyUpdate..., optimizer_op-inl.h:471-555,1305-1516):
-      // the updater sees (merged row_sparse, stored dense) and the key stays dense.  The rows are updated
-      // on every replica, each with its own complete optimizer state.
-      if (opt_.enabled && updater_ == nullptr && ks.state_world > 0) {
-        GatherState(ks);
-        ks.state_world = 0;
-        ks.state_devs.clear();
-      }
-    }
-  }
+  RowSparseKeyFor(ks);
   const int n_src = static_cast<int>(vals.size());
   MXKV_CHECK(n_src >= 1 && n_src <= kMaxSrc) << "push of " << n_src << " row_sparse values (max " << kMaxSrc << ")";
   const int64_t L = ks.size / ks.shape[0];
@@ -137,10 +285,7 @@ void KVStore::PushRowSparse(KeyState& ks, const std::vector<NDArray>& vals) {
     cap = std::max(cap, v.nnz());
   }
   const bool callback = updater_ != nullptr;
-  const bool fused = opt_.enabled && !callback;
-  if (fused)
-    MXKV_CHECK(opt_.kind == OPT_SGD || opt_.kind == OPT_SGD_MOM || opt_.kind == OPT_ADAM)
-        << "row_sparse gradients: only the lazy SGD / SGD-momentum / Adam updates are fused";
+  const bool fused = RowSparseFused();
 
   // ---- which GPUs compute (each one redundantly, on its own replica) -------------------------
   std::vector<int> work_devs;
@@ -184,130 +329,34 @@ void KVStore::PushRowSparse(KeyState& ks, const std::vector<NDArray>& vals) {
   const float wd = fused ? KeyWD(ks) : 0.f;
 
   // ---- MP: publish this rank's gradient in the symmetric staging area ---------------------------
-  int world = 1;
-  if (mp_mode && pg->world() > 1) {
-    world = pg->world();
+  const int world = mp_mode ? pg->world() : 1;
+  RspSources staged{};
+  if (world > 1) {
     Replica& r = *FindReplica(ks, pg->dev());
-    const int64_t stage_rows = std::min<int64_t>(ks.shape[0], EnvInt("MXKV_B200_RSP_STAGE_ROWS", 131072));
-    if (r.stage_idx.is_none()) {
-      const Context ctx{kGPU, pg->dev()};
-      r.stage_idx = NDArray::Empty({stage_rows}, ctx, kInt64, true);
-      r.stage_val = NDArray::Empty({stage_rows * L}, ctx, kFloat32, true);
-      r.stage_nnz = NDArray::Empty({2}, ctx, kInt64, true);
-    }
-    const NDArray& v = vals[0];
-    MXKV_CHECK(v.nnz() <= r.stage_idx.size())
-        << "row_sparse gradient with " << v.nnz() << " rows exceeds the staging capacity of "
-        << r.stage_idx.size() << " rows; raise MXKV_B200_RSP_STAGE_ROWS";
+    staged = PublishRowSparse(ks, r, vals[0], !fused_path);
     cap = r.stage_idx.size();
-    DeviceGuard g(pg->dev());
-    cudaStream_t s = rt->Dev(pg->dev()).stream;
-    // peers may still be reading the staging area of the previous push: rendezvous first
-    SyncArgs sync;
-    std::memset(&sync, 0, sizeof(sync));
-    sync.self = rt->Dev(pg->dev()).signal_pad;
-    for (int q = 0; q < world; ++q) sync.peers[q] = pg->signal_pad(q);
-    sync.world = world; sync.rank = pg->rank(); sync.mode = SYNC_WRITE_PEERS;
-    sync.timeout = rt->spin_timeout_cycles;
-    sync.epoch = rt->NextSyncEpoch(pg);
-    if (!fused_path || !r.rsp_stage_guarded) CheckLaunch(LaunchBarrier(sync, s), "barrier");
-    if (!fused_path) {
-      if (v.nnz() > 0) {
-        CopyBytes(v.idx_ptr(), v.ctx(), r.stage_idx.data(), r.stage_idx.ctx(), v.nnz() * 8);
-        CopyBytes(v.data(), v.ctx(), r.stage_val.data(), r.stage_val.ctx(), v.nnz() * L * 4);
-      }
-      CheckLaunch(LaunchSetI64(static_cast<int64_t*>(r.stage_nnz.data()), v.nnz(), s), "set_nnz");
-      sync.epoch = rt->NextSyncEpoch(pg);
-      CheckLaunch(LaunchBarrier(sync, s), "barrier");
-    }
-    r.rsp_stage_guarded = fused_path;      // the fused kernel ends with a cross-GPU barrier
   }
 
-  // ---- per computing GPU: sources as seen from it, then the four kernels -----------------------
+  // ---- per computing GPU: sources as seen from it, then the kernels ----------------------------
   for (int dev : work_devs) {
     Replica& r = *FindReplica(ks, dev);
     DeviceGuard g(dev);
     cudaStream_t s = rt->Dev(dev).stream;
-    RspSources S;
-    std::memset(&S, 0, sizeof(S));
     std::vector<void*> temps;
-    if (world > 1) {
-      S.n = world;
-      for (int q = 0; q < world; ++q) {
-        S.idx[q] = static_cast<const int64_t*>(r.stage_idx.peer_data(q));
-        S.val[q] = static_cast<const float*>(r.stage_val.peer_data(q));
-        S.nnz[q] = static_cast<const int64_t*>(r.stage_nnz.peer_data(q));
-      }
-    } else {
+    RspSources S = staged;
+    if (world == 1) {
       S.n = n_src;
-      for (int k = 0; k < n_src; ++k) {
-        const NDArray& v = vals[k];
-        const Context c = v.ctx();
-        const int64_t nnz = v.nnz();
-        const bool direct = c.is_gpu() && (c.dev_id == dev || rt->PeerOK(dev, c.dev_id));
-        if (direct) {
-          if (c.dev_id != dev) rt->StreamWait(dev, c.dev_id);
-          S.idx[k] = v.idx_ptr();
-          S.val[k] = static_cast<const float*>(v.data());
-          S.nnz[k] = v.d_nnz();
-        } else {   // host-resident (or unreachable) source: stage it on this GPU
-          void* ti = nullptr; void* tv = nullptr; int64_t* tn = nullptr;
-          CUDA_CALL(cudaMallocAsync(&ti, std::max<int64_t>(nnz, 1) * 8, s));
-          CUDA_CALL(cudaMallocAsync(&tv, std::max<int64_t>(nnz * L, 1) * 4, s));
-          CUDA_CALL(cudaMallocAsync(reinterpret_cast<void**>(&tn), 16, s));
-          if (nnz > 0) {
-            CopyBytes(v.idx_ptr(), c, ti, Context{kGPU, dev}, nnz * 8);
-            CopyBytes(v.data(), c, tv, Context{kGPU, dev}, nnz * L * 4);
-          }
-          CheckLaunch(LaunchSetI64(tn, nnz, s), "set_nnz");
-          temps.push_back(ti); temps.push_back(tv); temps.push_back(tn);
-          S.idx[k] = static_cast<const int64_t*>(ti);
-          S.val[k] = static_cast<const float*>(tv);
-          S.nnz[k] = tn;
-        }
-      }
-    }
-    if (!fused_path) EnsureRspWorkspace(ks, r, S.n, cap);      // (the fused kernel materialises no union)
-    RspRowArgs A;
-    std::memset(&A, 0, sizeof(A));
-    const bool std_update = fused && !opt_.lazy_update;   // dense pass over every row (reference default)
-    if (!fused_path) {
-      A.out_idx = r.rsp_merged.idx_ptr();
-      A.out_val = (fused && !std_update) ? nullptr : static_cast<float*>(r.rsp_merged.data());
-      A.d_nnz_out = r.rsp_merged.d_nnz();
-    }
-    A.table = static_cast<float*>(r.local.data());
-    A.row_len = L;
-    A.opt = (fused && !std_update) ? opt_.kind : OPT_NONE;
-    A.assign = (!fused && !callback) ? 1 : 0;
-    A.lr = lr; A.wd = wd; A.rescale = opt_.rescale; A.clip = opt_.clip; A.momentum = opt_.momentum;
-    A.beta1 = static_cast<float>(opt_.beta1); A.beta2 = static_cast<float>(opt_.beta2); A.eps = opt_.eps;
-    if (fused) {
-      A.s0 = r.s0.is_none() ? nullptr : static_cast<float*>(r.s0.data());
-      A.s1 = r.s1.is_none() ? nullptr : static_cast<float*>(r.s1.data());
-    }
-    bool vec = (L % 4 == 0) && Aligned16(A.table) && (A.out_val == nullptr || Aligned16(A.out_val)) &&
-               (A.s0 == nullptr || Aligned16(A.s0)) && (A.s1 == nullptr || Aligned16(A.s1));
-    for (int k = 0; k < S.n; ++k) vec = vec && Aligned16(S.val[k]);
-    A.vec = vec ? 1 : 0;
-    if (A.assign) {
-      // push without updater: local = merged (kvstore_local.h:279-284) -- rows outside the union vanish
-      CUDA_CALL(cudaMemsetAsync(r.local.data(), 0, r.local.nbytes(), s));
+      for (int k = 0; k < n_src; ++k) SourceOn(S, k, vals[k], L, dev, temps);
     }
     if (fused_path) {
+      RspRowArgs A = RowArgs(ks, r, S, false, true, false, lr, wd);    // (no union is materialised)
       RspStage St;
       std::memset(&St, 0, sizeof(St));
-      SyncArgs sync;
-      std::memset(&sync, 0, sizeof(sync));
-      sync.self = rt->Dev(dev).signal_pad;
-      sync.world = 1; sync.rank = 0; sync.mode = SYNC_NONE;
-      sync.timeout = rt->spin_timeout_cycles;
+      const SyncArgs sync = world > 1 ? GroupSync(SYNC_WRITE_PEERS) : LocalSync(dev);
       int64_t est_rows = 0;
       void* tmp_src[2] = {nullptr, nullptr};
       if (world > 1) {
         const NDArray& v = vals[0];
-        for (int q = 0; q < world; ++q) sync.peers[q] = pg->signal_pad(q);
-        sync.world = world; sync.rank = pg->rank(); sync.mode = SYNC_WRITE_PEERS;
         St.publish = 1;
         St.src_idx = v.idx_ptr();
         St.src_val = static_cast<const float*>(v.data());
@@ -347,36 +396,15 @@ void KVStore::PushRowSparse(KeyState& ks, const std::vector<NDArray>& vals) {
       }
       CheckLaunch(LaunchRspPushFused(dev, S, A, St, sync, est_rows, s), "rsp_push_fused");
       for (void* t : tmp_src) if (t) CUDA_CALL(cudaFreeAsync(t, s));
-      for (void* t : temps) CUDA_CALL(cudaFreeAsync(t, s));
-      r.fresh = true;
-      continue;
-    }
-    CheckLaunch(LaunchRspSum(S, A, static_cast<int32_t*>(r.rsp_first.data()),
-                             static_cast<int32_t*>(r.rsp_pf.data()), r.rsp_cap, s), "rsp_sum");
-    rt->launches += 3;
-    r.rsp_merged.set_nnz_device();
-    if (std_update) {
-      // densify the merged gradient (absent rows = 0) and run the dense kernel with the reference's
-      // "Std" arithmetic over the whole table: O(table), as in the reference
-      float* gd = nullptr;
-      CUDA_CALL(cudaMallocAsync(reinterpret_cast<void**>(&gd), static_cast<size_t>(ks.size) * 4, s));
-      CUDA_CALL(cudaMemsetAsync(gd, 0, static_cast<size_t>(ks.size) * 4, s));
-      CheckLaunch(LaunchRspScatter(gd, r.rsp_merged.idx_ptr(), r.rsp_merged.d_nnz(), r.rsp_merged.cap_rows(), L,
-                                   static_cast<const float*>(r.rsp_merged.data()), s), "rsp_scatter");
-      TensorWork tw = ReplicaWork(ks, r, false, 0, ks.size, lr, wd);
-      tw.src[0] = gd; tw.n_src = 1;
-      tw.out[0] = r.local.data(); tw.n_out = 1;
-      tw.flags = ks.size % 4 == 0 ? WorkFlags(tw, false) : 0;   // (tables of other sizes keep the scalar path)
-      const int kind = opt_.kind == OPT_SGD ? OPT_SGD_STD : (opt_.kind == OPT_ADAM ? OPT_ADAM_STD : opt_.kind);
-      LaunchLocal(LaunchClassKey{SYNC_NONE, kFloat32, 0}, tw, kind, dev);
-      CUDA_CALL(cudaFreeAsync(gd, s));
+    } else {
+      MergeRows(ks, r, S, cap, fused, !fused && !callback, lr, wd);
     }
     for (void* t : temps) CUDA_CALL(cudaFreeAsync(t, s));
     r.fresh = true;
   }
   if (world > 1) {
     // nobody may overwrite its staging area while a peer is still reading it: the rendezvous at the
-    // start of the next push (above) provides that ordering
+    // start of the next push (PublishRowSparse) provides that ordering
   } else {
     // sources on other GPUs were read by this GPU's kernels: they must not be reused earlier
     for (auto& v : vals) {
@@ -387,17 +415,7 @@ void KVStore::PushRowSparse(KeyState& ks, const std::vector<NDArray>& vals) {
   }
   if (callback) {
     Replica& root = *FindReplica(ks, work_devs[0]);
-    rt->Dev(root.dev).engine_dirty = true;
-    rt->Fence(root.dev);
-    NDHandle* recv = new NDHandle(root.rsp_merged);
-    NDHandle* local = new NDHandle(root.local);
-    if (key_type_ == kStringKey && str_updater_ != nullptr) {
-      str_updater_(reverse_str_key_dict_[ks.key].c_str(), recv, local, updater_handle_);
-    } else {
-      updater_(ks.key, recv, local, updater_handle_);
-    }
-    rt->AcquireUser(root.dev);
-    for (auto& r : ks.reps) r.fresh = (&r == &root);
+    RunCallbackUpdater(ks, root, root.rsp_merged);
   }
   for (int d : touched) rt->ReleaseToUser(d);
 }
@@ -419,27 +437,18 @@ void KVStore::HierPushRowSparse(KeyState& ks, const std::vector<NDArray>& vals) 
   MXKV_CHECK(nodes <= kMaxSrc) << "row_sparse push over " << nodes << " nodes (max " << kMaxSrc << ")";
   MXKV_CHECK(vals.size() == 1) << "one-process-per-GPU mode: push exactly one value per key per rank";
   const NDArray& v = vals[0];
-  if (ks.stype != kRowSparseStorage) {
-    MXKV_CHECK(ks.dtype == kFloat32 && !ks.shape.empty()) << "row_sparse values need a float32 key (key " << ks.key << ")";
-    if (ks.local_world > 0) GatherLocal(ks);
-    if (!opt_.enabled) ks.stype = kRowSparseStorage;
-    else if (ks.state_world > 0) { GatherState(ks); ks.state_world = 0; ks.state_devs.clear(); }
-  }
+  RowSparseKeyFor(ks);
   MXKV_CHECK(v.stype() == kRowSparseStorage && v.dtype() == kFloat32 && v.shape() == ks.shape)
       << "row_sparse push: storage type / shape / dtype mismatch for key " << ks.key;
-  const bool fused = opt_.enabled;
-  if (fused)
-    MXKV_CHECK(opt_.kind == OPT_SGD || opt_.kind == OPT_SGD_MOM || opt_.kind == OPT_ADAM)
-        << "row_sparse gradients: only the lazy SGD / SGD-momentum / Adam updates are fused";
-  const int world = pg->world(), dev = pg->dev();
+  const bool fused = RowSparseFused();
+  const int dev = pg->dev();
   const int64_t L = ks.size / ks.shape[0];
   DeviceGuard g(dev);
   cudaStream_t s = rt->Dev(dev).stream;
   rt->AcquireUser(dev);
   MXKV_CHECK(!v.ctx().is_gpu() || v.ctx().dev_id == dev) << "value must live on GPU " << dev << " or on the host";
   PublishNnz(v);
-  EnsureReplica(ks, dev);
-  Replica& r = *FindReplica(ks, dev);
+  Replica& r = EnsureReplica(ks, dev);
   if (fused) { EnsureState(ks, r, false); SyncState(ks, r); ks.count += 1; }
   const float lr = fused ? KeyLR(ks) : 0.f;
   const float wd = fused ? KeyWD(ks) : 0.f;
@@ -447,76 +456,16 @@ void KVStore::HierPushRowSparse(KeyState& ks, const std::vector<NDArray>& vals) 
 
   // ---- (1) the node's merge ---------------------------------------------------------------------------------
   RspSources S;
-  std::memset(&S, 0, sizeof(S));
   int64_t cap = std::max<int64_t>(v.nnz(), 1);
-  SyncArgs sync;
-  std::memset(&sync, 0, sizeof(sync));
-  if (world > 1) {
-    const int64_t stage_rows = std::min<int64_t>(ks.shape[0], EnvInt("MXKV_B200_RSP_STAGE_ROWS", 131072));
-    if (r.stage_idx.is_none()) {
-      const Context ctx{kGPU, dev};
-      r.stage_idx = NDArray::Empty({stage_rows}, ctx, kInt64, true);
-      r.stage_val = NDArray::Empty({stage_rows * L}, ctx, kFloat32, true);
-      r.stage_nnz = NDArray::Empty({2}, ctx, kInt64, true);
-    }
-    MXKV_CHECK(v.nnz() <= r.stage_idx.size())
-        << "row_sparse gradient with " << v.nnz() << " rows exceeds the staging capacity of " << r.stage_idx.size()
-        << " rows; raise MXKV_B200_RSP_STAGE_ROWS";
+  if (pg->world() > 1) {
+    S = PublishRowSparse(ks, r, v, true);
     cap = r.stage_idx.size();
-    sync.self = rt->Dev(dev).signal_pad;
-    for (int q = 0; q < world; ++q) sync.peers[q] = pg->signal_pad(q);
-    sync.world = world; sync.rank = pg->rank(); sync.mode = SYNC_WRITE_PEERS;
-    sync.timeout = rt->spin_timeout_cycles;
-    sync.epoch = rt->NextSyncEpoch(pg);
-    CheckLaunch(LaunchBarrier(sync, s), "barrier");      // peers are done with the previous push's staging
-    if (v.nnz() > 0) {
-      CopyBytes(v.idx_ptr(), v.ctx(), r.stage_idx.data(), r.stage_idx.ctx(), v.nnz() * 8);
-      CopyBytes(v.data(), v.ctx(), r.stage_val.data(), r.stage_val.ctx(), v.nnz() * L * 4);
-    }
-    CheckLaunch(LaunchSetI64(static_cast<int64_t*>(r.stage_nnz.data()), v.nnz(), s), "set_nnz");
-    sync.epoch = rt->NextSyncEpoch(pg);
-    CheckLaunch(LaunchBarrier(sync, s), "barrier");
-    S.n = world;
-    for (int q = 0; q < world; ++q) {
-      S.idx[q] = static_cast<const int64_t*>(r.stage_idx.peer_data(q));
-      S.val[q] = static_cast<const float*>(r.stage_val.peer_data(q));
-      S.nnz[q] = static_cast<const int64_t*>(r.stage_nnz.peer_data(q));
-    }
   } else {
+    std::memset(&S, 0, sizeof(S));
     S.n = 1;
-    if (v.ctx().is_gpu()) {
-      S.idx[0] = v.idx_ptr(); S.val[0] = static_cast<const float*>(v.data()); S.nnz[0] = v.d_nnz();
-    } else {
-      void* ti = nullptr; void* tv = nullptr; int64_t* tn = nullptr;
-      CUDA_CALL(cudaMallocAsync(&ti, cap * 8, s));
-      CUDA_CALL(cudaMallocAsync(&tv, std::max<int64_t>(cap * L, 1) * 4, s));
-      CUDA_CALL(cudaMallocAsync(reinterpret_cast<void**>(&tn), 16, s));
-      if (v.nnz() > 0) {
-        CopyBytes(v.idx_ptr(), v.ctx(), ti, Context{kGPU, dev}, v.nnz() * 8);
-        CopyBytes(v.data(), v.ctx(), tv, Context{kGPU, dev}, v.nnz() * L * 4);
-      }
-      CheckLaunch(LaunchSetI64(tn, v.nnz(), s), "set_nnz");
-      temps.push_back(ti); temps.push_back(tv); temps.push_back(tn);
-      S.idx[0] = static_cast<const int64_t*>(ti); S.val[0] = static_cast<const float*>(tv); S.nnz[0] = tn;
-    }
+    SourceOn(S, 0, v, L, dev, temps);
   }
-  EnsureRspWorkspace(ks, r, S.n, cap);
-  RspRowArgs A;
-  std::memset(&A, 0, sizeof(A));
-  A.out_idx = r.rsp_merged.idx_ptr();
-  A.out_val = static_cast<float*>(r.rsp_merged.data());
-  A.d_nnz_out = r.rsp_merged.d_nnz();
-  A.table = static_cast<float*>(r.local.data());
-  A.row_len = L;
-  A.opt = OPT_NONE;
-  A.assign = 0;
-  bool vec = (L % 4 == 0) && Aligned16(A.table) && Aligned16(A.out_val);
-  for (int k = 0; k < S.n; ++k) vec = vec && Aligned16(S.val[k]);
-  A.vec = vec ? 1 : 0;
-  CheckLaunch(LaunchRspSum(S, A, static_cast<int32_t*>(r.rsp_first.data()), static_cast<int32_t*>(r.rsp_pf.data()),
-                           r.rsp_cap, s), "rsp_sum");
-  rt->launches += 3;
-  r.rsp_merged.set_nnz_device();
+  MergeRows(ks, r, S, cap, false, false, lr, wd);
 
   // ---- (2) gather the nodes' merged gradients ------------------------------------------------------------------
   int64_t* cnt = nullptr;                  // [nodes] row counts, device
@@ -556,46 +505,7 @@ void KVStore::HierPushRowSparse(KeyState& ks, const std::vector<NDArray>& vals) 
     S2.val[q] = val_all + static_cast<size_t>(q) * cap2 * L;
     S2.nnz[q] = cnt + q;
   }
-  EnsureRspWorkspace(ks, r, nodes, cap2);
-  const bool std_update = fused && !opt_.lazy_update;
-  RspRowArgs B;
-  std::memset(&B, 0, sizeof(B));
-  B.out_idx = r.rsp_merged.idx_ptr();
-  B.out_val = (fused && !std_update) ? nullptr : static_cast<float*>(r.rsp_merged.data());
-  B.d_nnz_out = r.rsp_merged.d_nnz();
-  B.table = static_cast<float*>(r.local.data());
-  B.row_len = L;
-  B.opt = (fused && !std_update) ? opt_.kind : OPT_NONE;
-  B.assign = fused ? 0 : 1;
-  B.lr = lr; B.wd = wd; B.rescale = opt_.rescale; B.clip = opt_.clip; B.momentum = opt_.momentum;
-  B.beta1 = static_cast<float>(opt_.beta1); B.beta2 = static_cast<float>(opt_.beta2); B.eps = opt_.eps;
-  if (fused) {
-    B.s0 = r.s0.is_none() ? nullptr : static_cast<float*>(r.s0.data());
-    B.s1 = r.s1.is_none() ? nullptr : static_cast<float*>(r.s1.data());
-  }
-  bool vec2 = (L % 4 == 0) && Aligned16(B.table) && (B.out_val == nullptr || Aligned16(B.out_val)) &&
-              (B.s0 == nullptr || Aligned16(B.s0)) && (B.s1 == nullptr || Aligned16(B.s1));
-  for (int q = 0; q < nodes; ++q) vec2 = vec2 && Aligned16(S2.val[q]);
-  B.vec = vec2 ? 1 : 0;
-  if (B.assign) CUDA_CALL(cudaMemsetAsync(r.local.data(), 0, r.local.nbytes(), s));   // local = merged
-  CheckLaunch(LaunchRspSum(S2, B, static_cast<int32_t*>(r.rsp_first.data()), static_cast<int32_t*>(r.rsp_pf.data()),
-                           r.rsp_cap, s), "rsp_sum");
-  rt->launches += 3;
-  r.rsp_merged.set_nnz_device();
-  if (std_update) {
-    float* gd = nullptr;
-    CUDA_CALL(cudaMallocAsync(reinterpret_cast<void**>(&gd), static_cast<size_t>(ks.size) * 4, s));
-    CUDA_CALL(cudaMemsetAsync(gd, 0, static_cast<size_t>(ks.size) * 4, s));
-    CheckLaunch(LaunchRspScatter(gd, r.rsp_merged.idx_ptr(), r.rsp_merged.d_nnz(), r.rsp_merged.cap_rows(), L,
-                                 static_cast<const float*>(r.rsp_merged.data()), s), "rsp_scatter");
-    TensorWork tw = ReplicaWork(ks, r, false, 0, ks.size, lr, wd);
-    tw.src[0] = gd; tw.n_src = 1;
-    tw.out[0] = r.local.data(); tw.n_out = 1;
-    tw.flags = ks.size % 4 == 0 ? WorkFlags(tw, false) : 0;   // (tables of other sizes keep the scalar path)
-    const int kind = opt_.kind == OPT_SGD ? OPT_SGD_STD : (opt_.kind == OPT_ADAM ? OPT_ADAM_STD : opt_.kind);
-    LaunchLocal(LaunchClassKey{SYNC_NONE, kFloat32, 0}, tw, kind, dev);
-    CUDA_CALL(cudaFreeAsync(gd, s));
-  }
+  MergeRows(ks, r, S2, cap2, fused, !fused, lr, wd);
   for (void* t : temps) CUDA_CALL(cudaFreeAsync(t, s));
   r.fresh = true;
   ks.local_world = 0;
@@ -685,13 +595,8 @@ void KVStore::PullRowSparseImpl(const std::vector<int>& keys,
     const int vec = (L % 4 == 0 && Aligned16(r.local.data()) && Aligned16(target.data())) ? 1 : 0;
     if (n >= 1 && n <= RspUniqueMax() && EnvInt("MXKV_B200_RSP_FUSED", 1) != 0) {
       // unique | grid barrier | gather in one launch
-      SyncArgs sync;
-      std::memset(&sync, 0, sizeof(sync));
-      sync.self = rt->Dev(dev).signal_pad;
-      sync.world = 1; sync.rank = 0; sync.mode = SYNC_NONE;
-      sync.timeout = rt->spin_timeout_cycles;
       CheckLaunch(LaunchRspPullFused(dev, static_cast<const float*>(r.local.data()), ids, n, target.idx_ptr(),
-                                     target.d_nnz(), L, static_cast<float*>(target.data()), vec, sync, s),
+                                     target.d_nnz(), L, static_cast<float*>(target.data()), vec, LocalSync(dev), s),
                   "rsp_pull_fused");
     } else {
       CheckLaunch(LaunchRspUnique(ids, n, target.idx_ptr(), target.d_nnz(), s), "rsp_unique");

@@ -64,17 +64,21 @@ def test_row_sparse_pull_retain():
         assert _bits_equal(dense[r], table[r] if r in ids else np.zeros(L, np.float32))
 
 
-@pytest.mark.parametrize("lazy", [True, False])
+@pytest.mark.parametrize("lazy", [True, False, "four-kernel"])
 @pytest.mark.parametrize("optname,kw", [
     ("sgd", dict(learning_rate=0.1, wd=1e-3, rescale_grad=0.5, clip_gradient=0.6)),
     ("sgd", dict(learning_rate=0.1, wd=1e-3, momentum=0.9)),
     ("adam", dict(learning_rate=0.01, wd=1e-3)),
 ])
-def test_fused_sparse_update(optname, kw, lazy):
+def test_fused_sparse_update(optname, kw, lazy, monkeypatch):
     """lazy_update=True: only the rows present in the summed gradient are touched (SGDDnsRspKernel /
     SGDMomDnsRspDnsKernel / AdamDnsRspDnsKernel); lazy_update=False (the reference default): the
     standard update over every row (SGDUpdateDnsRspImpl non-lazy branch, SGDMomStdDnsRspDnsKernel,
-    AdamStdDnsRspDnsKernel)."""
+    AdamStdDnsRspDnsKernel).  "four-kernel": the lazy update with MXKV_B200_RSP_FUSED=0, run by the union +
+    gather-sum kernels (the code of the multi-node push's final merge) instead of rsp_push_fused_kernel."""
+    if lazy == "four-kernel":
+        monkeypatch.setenv("MXKV_B200_RSP_FUSED", "0")
+        lazy = True
     kw = dict(kw, lazy_update=lazy)
     rng = np.random.default_rng(11)
     rows, L, nnz, n = 2000, 64, 150, 4
@@ -156,6 +160,13 @@ def test_sp_multi_gpu_sources():
             want = O.sparse_retain(okv.local[0], O.unique(ids))
             assert np.array_equal(out.indices.asnumpy(), want.indices)
             assert _bits_equal(out.data.asnumpy(), want.data.reshape(-1, L)), (step, d)
+
+
+@pytest.mark.multigpu
+def test_sp_multi_gpu_sources_four_kernel_path(monkeypatch):
+    """The same with MXKV_B200_RSP_FUSED=0 (peer sources read by the union + gather-sum kernels)."""
+    monkeypatch.setenv("MXKV_B200_RSP_FUSED", "0")
+    test_sp_multi_gpu_sources()
 
 
 @pytest.mark.parametrize("n", [1, 4])
