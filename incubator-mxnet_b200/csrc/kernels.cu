@@ -100,7 +100,7 @@ __device__ __forceinline__ void process_packets(const TensorWork& tw, const int6
         pw.load(tw.w, e[u]);
         pw.unpack(w[u]);
       }
-      if (OPT == OPT_SGD_MOM || OPT == OPT_ADAM || OPT == OPT_ADAMW || OPT == OPT_ADAM_STD) ldf<N>(tw.s0, e[u], s0[u]);
+      if (OPT == OPT_SGD_MOM || OPT == OPT_ADAM || OPT == OPT_ADAMW || OPT == OPT_ADAM_STD || OPT == OPT_NAG) ldf<N>(tw.s0, e[u], s0[u]);
       if (OPT == OPT_ADAM || OPT == OPT_ADAMW || OPT == OPT_ADAM_STD) ldf<N>(tw.s1, e[u], s1[u]);
     }
 #pragma unroll
@@ -108,7 +108,7 @@ __device__ __forceinline__ void process_packets(const TensorWork& tw, const int6
       if (!ok[u]) continue;
 #pragma unroll
       for (int i = 0; i < N; ++i) wnew[u][i] = update_one<OPT>(acc[u][i], w[u][i], s0[u][i], s1[u][i], h);
-      if (OPT == OPT_SGD_MOM || OPT == OPT_ADAM || OPT == OPT_ADAMW || OPT == OPT_ADAM_STD) stf<N>(tw.s0, e[u], s0[u]);
+      if (OPT == OPT_SGD_MOM || OPT == OPT_ADAM || OPT == OPT_ADAMW || OPT == OPT_ADAM_STD || OPT == OPT_NAG) stf<N>(tw.s0, e[u], s0[u]);
       if (OPT == OPT_ADAM || OPT == OPT_ADAMW || OPT == OPT_ADAM_STD) stf<N>(tw.s1, e[u], s1[u]);
       if (MP) stf<N>(tw.w32, e[u], wnew[u]);
     }
@@ -155,6 +155,7 @@ kv_dense_kernel(DenseLaunch L) {
     h.lr = tw.lr; h.wd = tw.wd; h.eta = tw.eta;
     h.rescale = L.rescale; h.clip = L.clip; h.momentum = L.momentum;
     h.beta1 = L.beta1; h.beta2 = L.beta2; h.eps = L.eps;
+    h.mp = sizeof(T) == 2 && L.mp_arith != 0;
 
     const int64_t cb = tw.begin + (c - L.chunk_prefix[lo]) * L.chunk_elems;
     const int64_t ce = (cb + L.chunk_elems < tw.end) ? cb + L.chunk_elems : tw.end;
@@ -250,7 +251,7 @@ kv_dense_bulk_kernel(DenseLaunch L) {
   const uint32_t arr_bytes = static_cast<uint32_t>(tile) * 4u;
   const uint32_t stage_bytes = arr_bytes * static_cast<uint32_t>(L.bulk_arrays);
   constexpr bool HAS_W = OPT != OPT_NONE;
-  constexpr bool HAS_S0 = OPT == OPT_SGD_MOM || OPT == OPT_ADAM || OPT == OPT_ADAMW;
+  constexpr bool HAS_S0 = OPT == OPT_SGD_MOM || OPT == OPT_ADAM || OPT == OPT_ADAMW || OPT == OPT_NAG;
   constexpr bool HAS_S1 = OPT == OPT_ADAM || OPT == OPT_ADAMW;
 
   if (threadIdx.x == 0) {
@@ -342,6 +343,7 @@ kv_dense_bulk_kernel(DenseLaunch L) {
     h.lr = tw.lr; h.wd = tw.wd; h.eta = tw.eta;
     h.rescale = L.rescale; h.clip = L.clip; h.momentum = L.momentum;
     h.beta1 = L.beta1; h.beta2 = L.beta2; h.eps = L.eps;
+    h.mp = false;                     // float32 keys only
     const int64_t cb = tw.begin + (c - L.chunk_prefix[lo]) * tile;
     const int64_t ce = (cb + tile < tw.end) ? cb + tile : tw.end;
     const int nvec = static_cast<int>((ce - cb) >> 2);
@@ -415,6 +417,7 @@ static BulkKernelFn pick_bulk(int opt, int mp) {
     case OPT_ADAM: return mp ? kv_dense_bulk_kernel<OPT_ADAM, true> : kv_dense_bulk_kernel<OPT_ADAM, false>;
     case OPT_ADAMW: return mp ? kv_dense_bulk_kernel<OPT_ADAMW, true> : kv_dense_bulk_kernel<OPT_ADAMW, false>;
     case OPT_TEST: return mp ? kv_dense_bulk_kernel<OPT_TEST, true> : kv_dense_bulk_kernel<OPT_TEST, false>;
+    case OPT_NAG: return mp ? kv_dense_bulk_kernel<OPT_NAG, true> : kv_dense_bulk_kernel<OPT_NAG, false>;
     default: return nullptr;
   }
 }
@@ -495,7 +498,7 @@ __global__ void __launch_bounds__(kThreads, (U >= 4 || PIPE) ? 1 : 2)
 kv_dense_nvls_kernel(DenseLaunch L) {
   __shared__ TensorWork tw;
   barrier_start(L.sync);
-  constexpr bool HAS_S0 = OPT == OPT_SGD_MOM || OPT == OPT_ADAM || OPT == OPT_ADAMW;
+  constexpr bool HAS_S0 = OPT == OPT_SGD_MOM || OPT == OPT_ADAM || OPT == OPT_ADAMW || OPT == OPT_NAG;
   constexpr bool HAS_S1 = OPT == OPT_ADAM || OPT == OPT_ADAMW;
   int cur = -1;
   int64_t c = blockIdx.x;
@@ -524,6 +527,7 @@ kv_dense_nvls_kernel(DenseLaunch L) {
     h.lr = tw.lr; h.wd = tw.wd; h.eta = tw.eta;
     h.rescale = L.rescale; h.clip = L.clip; h.momentum = L.momentum;
     h.beta1 = L.beta1; h.beta2 = L.beta2; h.eps = L.eps;
+    h.mp = false;                     // float32 keys only
     const int64_t nvec = (k.ce - k.cb) >> 2;
     const int n_plain = tw.n_out - tw.n_mc;
     // state of all U packets first (independent HBM loads in flight together), then the arithmetic
@@ -581,6 +585,7 @@ static NvlsKernelFn pick_nvls_opt(int opt, int mp) {
     case OPT_ADAM: return mp ? kv_dense_nvls_kernel<OPT_ADAM, true, U, PIPE> : kv_dense_nvls_kernel<OPT_ADAM, false, U, PIPE>;
     case OPT_ADAMW: return mp ? kv_dense_nvls_kernel<OPT_ADAMW, true, U, PIPE> : kv_dense_nvls_kernel<OPT_ADAMW, false, U, PIPE>;
     case OPT_TEST: return mp ? kv_dense_nvls_kernel<OPT_TEST, true, U, PIPE> : kv_dense_nvls_kernel<OPT_TEST, false, U, PIPE>;
+    case OPT_NAG: return mp ? kv_dense_nvls_kernel<OPT_NAG, true, U, PIPE> : kv_dense_nvls_kernel<OPT_NAG, false, U, PIPE>;
     default: return nullptr;
   }
 }
@@ -681,6 +686,7 @@ static DenseKernelFn pick_opt(int opt, bool mp, bool small_n, bool allow_non_mp)
       case OPT_ADAM: return pick_n<T, OPT_ADAM, true>(small_n);
       case OPT_ADAMW: return pick_n<T, OPT_ADAMW, true>(small_n);
       case OPT_TEST: return pick_n<T, OPT_TEST, true>(small_n);
+      case OPT_NAG: return pick_n<T, OPT_NAG, true>(small_n);
       default: return nullptr;
     }
   }
@@ -701,6 +707,7 @@ static DenseKernelFn pick_kernel(const DenseLaunch& L) {
         case OPT_ADAM: return pick_n<float, OPT_ADAM, false>(sn);
         case OPT_ADAMW: return pick_n<float, OPT_ADAMW, false>(sn);
         case OPT_TEST: return pick_n<float, OPT_TEST, false>(sn);
+        case OPT_NAG: return pick_n<float, OPT_NAG, false>(sn);
         case OPT_SGD_STD: return kv_dense_kernel<float, OPT_SGD_STD, false, false>;
         case OPT_ADAM_STD: return kv_dense_kernel<float, OPT_ADAM_STD, false, false>;
         default: return nullptr;
@@ -740,9 +747,9 @@ int DenseMaxGrid(int device, int threads) {
 // Function attributes are per device: opt in to large dynamic shared memory on the GPU a launch goes to -- and
 // only there (a process that owns one GPU must not create contexts on the others).  The device must be current.
 static bool EnsureBulkAttr(int device, int opt, int multi_precision) {
-  static bool attr_done[64][16] = {{false}};
-  if (device < 0 || device >= 64) return false;
-  const int slot = (opt & 7) * 2 + (multi_precision ? 1 : 0);
+  static bool attr_done[64][32] = {{false}};
+  if (device < 0 || device >= 64 || opt < 0 || opt >= 16) return false;
+  const int slot = opt * 2 + (multi_precision ? 1 : 0);
   if (attr_done[device][slot]) return true;
   BulkKernelFn fn = pick_bulk(opt, multi_precision);
   if (fn == nullptr) return false;

@@ -39,7 +39,8 @@ enum OptKind : int {
   // layer-wise adaptive optimizers: need per-tensor norms, run as a launch sequence (norm_kernels.h)
   OPT_LAMB = 8,     // multi_lamb_update / multi_mp_lamb_update   contrib/multi_lamb.cc:36-120
   OPT_LANS = 9,     // multi_lans_update / multi_mp_lans_update   contrib/multi_lans.cc:36-130
-  OPT_LARS = 10     // LARS._get_lars + (mp_)sgd(_mom)_update     python/mxnet/optimizer/lars.py:117-133,244-275
+  OPT_LARS = 10,    // LARS._get_lars + (mp_)sgd(_mom)_update     python/mxnet/optimizer/lars.py:117-133,244-275
+  OPT_NAG = 11      // NAGMomKernel / MP_NAGMomKernel        optimizer_op-inl.h:1029-1044,1066-1090
 };
 inline bool IsNormOpt(int kind) { return kind == OPT_LAMB || kind == OPT_LANS || kind == OPT_LARS; }
 
@@ -144,6 +145,8 @@ struct DenseLaunch {
   int bulk_group;                // consecutive tiles a block takes before it strides on by grid * bulk_group tiles
   int nvls_unroll;               // NVLS variant: multimem.ld_reduce requests in flight per thread (1, 2, 4 or 8)
   int nvls_pipe;                 // NVLS variant: 1 = next chunk's ld_reduce issued before this chunk's update/stores
+  int mp_arith;                  // 1: a 16-bit key of an optimizer created with multi_precision -- update_one takes
+                                 //   the mp_* operator's grouping where it differs from the plain one (Hyper::mp)
 };
 
 // returns cudaError_t as int; never throws

@@ -434,6 +434,7 @@ void KVStore::SetOptimizer(const std::string& name, const std::vector<std::pair<
   else if (n == "lamb") { c.kind = OPT_LAMB; c.lr = 0.001; c.eps = 1e-6f; }    // lamb.py:66-68
   else if (n == "lans") { c.kind = OPT_LANS; c.lr = 0.001; c.eps = 1e-6f; }    // lans.py:61-63
   else if (n == "lars") { c.kind = OPT_LARS; c.lr = 0.1; }                     // lars.py:77-79
+  else if (n == "nag") { c.kind = OPT_NAG; c.lr = 0.1; c.momentum = 0.9f; }     // nag.py:58
   else MXKV_FATAL() << "optimizer '" << name << "' has no fused kernel; register a Python updater instead";
   for (auto& kv : kwargs) {
     const std::string& k = kv.first;
@@ -461,6 +462,7 @@ void KVStore::SetOptimizer(const std::string& name, const std::vector<std::pair<
     else MXKV_FATAL() << "unknown optimizer argument '" << k << "'";
   }
   if (c.kind == OPT_SGD && c.momentum != 0.f) c.kind = OPT_SGD_MOM;   // sgd.py:213-224
+  if (c.kind == OPT_NAG && c.momentum == 0.f) c.kind = OPT_SGD;       // nag.py:59-63,141-154: no state, (mp_)sgd_update
   MXKV_CHECK(!c.skip_nonfinite || IsNormOpt(c.kind)) << "skip_nonfinite is available for lamb / lans / lars";
   c.lr_mult = opt_.lr_mult;
   c.wd_mult = opt_.wd_mult;
@@ -649,7 +651,7 @@ void KVStore::EnsureState(KeyState& ks, Replica& r, bool mp) {
   DeviceGuard g(r.dev);
   cudaStream_t s = rt->Dev(r.dev).stream;
   const bool need_s0 = opt_.kind == OPT_SGD_MOM || opt_.kind == OPT_ADAM || opt_.kind == OPT_ADAMW ||
-                       opt_.kind == OPT_LAMB || opt_.kind == OPT_LANS ||
+                       opt_.kind == OPT_NAG || opt_.kind == OPT_LAMB || opt_.kind == OPT_LANS ||
                        (opt_.kind == OPT_LARS && opt_.momentum != 0.f);      // lars.py:96-101
   const bool need_s1 = opt_.kind == OPT_ADAM || opt_.kind == OPT_ADAMW || opt_.kind == OPT_LAMB || opt_.kind == OPT_LANS;
   if (IsNormOpt(opt_.kind)) {
@@ -2129,7 +2131,8 @@ void KVStore::LaunchWorks(const LaunchClassKey& ck, std::vector<std::vector<Tens
     for (int p = my_first; p <= my_last; ++p)
       for (auto& t : per_part[p]) { ok = ok && (t.flags & kWorkStaged); max_src = std::max(max_src, t.n_src); }
     const int extra = (opt_kind != OPT_NONE ? 1 : 0) +
-                      ((opt_kind == OPT_SGD_MOM || opt_kind == OPT_ADAM || opt_kind == OPT_ADAMW) ? 1 : 0) +
+                      ((opt_kind == OPT_SGD_MOM || opt_kind == OPT_ADAM || opt_kind == OPT_ADAMW ||
+                        opt_kind == OPT_NAG) ? 1 : 0) +
                       ((opt_kind == OPT_ADAM || opt_kind == OPT_ADAMW) ? 1 : 0);
     // the staged variant is taken (a) whenever sources are read over NVLink (more bytes in flight
     // against a ~2 us round trip) and (b) locally when a thread of the per-thread variant would have
@@ -2187,6 +2190,9 @@ void KVStore::LaunchWorks(const LaunchClassKey& ck, std::vector<std::vector<Tens
     L.dtype = ck.dtype;
     L.opt = opt_kind;
     L.multi_precision = ck.mp;
+    // nag.py:137: mp_nag_mom_update where the optimizer asked for multi_precision on a 16-bit key
+    L.mp_arith = (opt_kind != OPT_NONE && opt_.multi_precision &&
+                  (ck.dtype == kFloat16 || ck.dtype == kBfloat16)) ? 1 : 0;
     L.order = ck.tree ? ORDER_TREE : order_;
     L.fp32_accum = (opt_kind != OPT_NONE || ck.dtype == kBfloat16 ||
                     EnvInt("MXKV_B200_FP16_FP32_ACCUM", 0) != 0) ? 1 : 0;

@@ -25,6 +25,7 @@ namespace mxkv {
 
 struct Hyper {
   float lr, wd, eta, rescale, clip, momentum, beta1, beta2, eps;
+  bool mp;    // OPT_NAG only: MP_NAGMomKernel's grouping of the weight step (DenseLaunch::mp_arith)
 };
 
 MXKV_HD float clipf(float x, float b) {   // mshadow_op::clip, mshadow_op.h:999-1009
@@ -86,6 +87,16 @@ MXKV_HD float update_one(float g, float w, float& s0, float& s1, const Hyper& h)
     const float v = __fadd_rn(__fmul_rn(h.beta2, s1), __fmul_rn(__fsub_rn(1.f, h.beta2), __fmul_rn(r, r)));
     s0 = m; s1 = v;
     return __fsub_rn(w, __fdiv_rn(__fmul_rn(h.lr, m), __fadd_rn(__fsqrt_rn(v), h.eps)));
+  } else if (OPT == OPT_NAG) {
+    float r = __fmul_rn(h.rescale, g);
+    if (h.clip >= 0.0f) r = clipf(r, h.clip);
+    r = __fadd_rn(r, __fmul_rn(h.wd, w));
+    float m = __fmul_rn(s0, h.momentum);
+    m = __fsub_rn(m, __fmul_rn(h.lr, r));
+    s0 = m;
+    // NAGMomKernel: (w + momentum*mom) - lr*r;  MP_NAGMomKernel: w + (momentum*mom - lr*r)
+    if (h.mp) return __fadd_rn(w, __fsub_rn(__fmul_rn(h.momentum, m), __fmul_rn(h.lr, r)));
+    return __fsub_rn(__fadd_rn(w, __fmul_rn(h.momentum, m)), __fmul_rn(h.lr, r));
   }
   return g;  // OPT_NONE
 }

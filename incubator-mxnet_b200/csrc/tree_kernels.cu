@@ -63,7 +63,7 @@ __device__ __forceinline__ void tree_packet(const TensorWork& tw, int64_t e, con
 #pragma unroll
     for (int i = 0; i < N; ++i) wnew[i] = acc[i];
   } else {
-    constexpr bool HAS_S0 = OPT == OPT_SGD_MOM || OPT == OPT_ADAM || OPT == OPT_ADAMW;
+    constexpr bool HAS_S0 = OPT == OPT_SGD_MOM || OPT == OPT_ADAM || OPT == OPT_ADAMW || OPT == OPT_NAG;
     constexpr bool HAS_S1 = OPT == OPT_ADAM || OPT == OPT_ADAMW;
     float w[N], s0[N], s1[N];
     if (MP) {
@@ -124,6 +124,7 @@ kv_dense_tree_kernel(DenseLaunch L) {
     h.lr = tw.lr; h.wd = tw.wd; h.eta = tw.eta;
     h.rescale = L.rescale; h.clip = L.clip; h.momentum = L.momentum;
     h.beta1 = L.beta1; h.beta2 = L.beta2; h.eps = L.eps;
+    h.mp = sizeof(T) == 2 && L.mp_arith != 0;
 
     const int64_t cb = tw.begin + (c - L.chunk_prefix[lo]) * L.chunk_elems;
     const int64_t ce = (cb + L.chunk_elems < tw.end) ? cb + L.chunk_elems : tw.end;
@@ -184,6 +185,7 @@ static TreeKernelFn pick_tree_opt(int opt, bool mp, bool allow_non_mp) {
       case OPT_ADAM: return kv_dense_tree_kernel<T, OPT_ADAM, true>;
       case OPT_ADAMW: return kv_dense_tree_kernel<T, OPT_ADAMW, true>;
       case OPT_TEST: return kv_dense_tree_kernel<T, OPT_TEST, true>;
+      case OPT_NAG: return kv_dense_tree_kernel<T, OPT_NAG, true>;
       default: return nullptr;
     }
   }
@@ -195,6 +197,7 @@ static TreeKernelFn pick_tree_opt(int opt, bool mp, bool allow_non_mp) {
       case OPT_ADAM: return kv_dense_tree_kernel<T, OPT_ADAM, false>;
       case OPT_ADAMW: return kv_dense_tree_kernel<T, OPT_ADAMW, false>;
       case OPT_TEST: return kv_dense_tree_kernel<T, OPT_TEST, false>;
+      case OPT_NAG: return kv_dense_tree_kernel<T, OPT_NAG, false>;
       default: return nullptr;
     }
   }

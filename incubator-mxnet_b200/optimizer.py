@@ -2,7 +2,7 @@
 
 Two roles:
 * describe the hyper-parameters of the optimizers that have a fused kernel in the native
-  engine (SGD / SGD-momentum / multi-precision SGD, Adam, AdamW, Test, and the layer-wise adaptive
+  engine (SGD / SGD-momentum / multi-precision SGD, NAG, Adam, AdamW, Test, and the layer-wise adaptive
   LAMB / LANS / LARS) -- ``KVStore.set_optimizer``
   hands them to ``MXKVB200SetOptimizer`` and the update then runs inside the reduce kernel;
 * provide the generic ``Updater`` callback (updater.py:39-93) for any other Optimizer object:
@@ -239,6 +239,44 @@ class SGD(Optimizer):
                 w.add_(state)
             else:
                 w.sub_(lr * g)
+
+
+@register
+class NAG(Optimizer):
+    """python/mxnet/optimizer/nag.py: Nesterov accelerated gradient; fused kernels nag_mom_update /
+    mp_nag_mom_update (src/operator/optimizer_op-inl.h:1029-1092), sgd_update / mp_sgd_update at momentum 0::
+
+        grad = clip(grad * rescale_grad, clip_gradient) + wd * weight
+        mom = momentum * mom - lr * grad
+        weight = weight + momentum * mom - lr * grad
+    """
+    fused_name = "nag"
+
+    def __init__(self, learning_rate=0.1, momentum=0.9, multi_precision=False, **kwargs):
+        super(NAG, self).__init__(learning_rate=learning_rate, multi_precision=multi_precision, **kwargs)
+        self.momentum = momentum
+
+    def fused_kwargs(self):
+        kw = super(NAG, self).fused_kwargs()
+        kw["momentum"] = self.momentum
+        return kw
+
+    def create_state(self, index, weight):
+        import torch
+        return torch.zeros_like(weight.as_torch(), dtype=torch.float32) if self.momentum != 0.0 else None
+
+    def step(self, indices, weights, grads, states):     # nag.py:72-109
+        for index, weight, grad, state in zip(indices, weights, grads, states):
+            self._update_count(index)
+            lr = self._get_lr(index)
+            w, g = weight.as_torch(), grad.as_torch()
+            g = _prep_grad(self, index, w, g)
+            if state is not None:
+                state.mul_(self.momentum).sub_(lr * g)
+                d = self.momentum * state - lr * g
+            else:
+                d = -lr * g
+            w.add_(d)
 
 
 @register
