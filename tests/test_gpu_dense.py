@@ -293,6 +293,12 @@ _OPTS = {
     "none": (None, {}),
     "sgd_mom": ("sgd", dict(learning_rate=0.01, momentum=0.9, wd=1e-4)),      # bench.py's optimizer
     "adam": ("adam", dict(learning_rate=0.001, wd=1e-3)),
+    "sgd": ("sgd", dict(learning_rate=0.1, wd=1e-4)),
+    "adamw": ("adamw", dict(learning_rate=0.001, wd=1e-2)),
+    "test": ("test", dict(learning_rate=0.1, wd=1e-3, rescale_grad=0.5)),
+    # n = 2 gradients in [-1, 1): |0.25 * sum| reaches 0.5, the clip at 0.1 binds on most elements
+    "adam_clip": ("adam", dict(learning_rate=0.01, wd=1e-3, rescale_grad=0.25, clip_gradient=0.1)),
+    "adamw_clip": ("adamw", dict(learning_rate=0.01, wd=1e-2, rescale_grad=0.25, clip_gradient=0.1)),
 }
 
 
@@ -322,15 +328,15 @@ def _fill(rng, lo, hi, e):
     return np.resize(rng.uniform(lo, hi, 1000003).astype(np.float32), e)
 
 
-def _run_keyset(variant, optkey, n, sizes, steps=2, seed=0):
+def _run_keyset(variant, optkey, n, sizes, steps=2, seed=0, kvtype="device"):
     optname, kw = _OPTS[optkey]
     rng = _rng(seed + n + len(sizes))
     keys = list(range(len(sizes)))
     w0 = [_fill(rng, 0, 1, e) for e in sizes]
     with _forced(variant) as f:
-        kv = mx.kv.create("device")
+        kv = mx.kv.create(kvtype)
         kv.init(keys, [mx.nd.array(w, mx.gpu(0)) for w in w0])
-        okv = O.OracleKVStore("device")
+        okv = O.OracleKVStore(kvtype)
         okv.init(keys, [w.copy() for w in w0])
         if optname:
             kv.set_optimizer(mx.optimizer.create(optname, **kw))
@@ -378,6 +384,19 @@ def test_forced_variant_ragged_tiles(variant):
     tiles of 4 elements, a key smaller than one tile next to a large one"""
     _run_keyset(variant, "sgd_mom", 2, [4, 2052, 8196, 3 * 2048 + 12, (1 << 20) + 4, 12], steps=3, seed=5)
     _run_keyset(variant, "adam", 1, [2048, 2044, 4096 + 8, 100004], steps=2, seed=6)
+
+
+@pytest.mark.parametrize("optkey", ["sgd", "adamw", "test", "adam_clip", "adamw_clip"])
+@pytest.mark.parametrize("variant", ["bulk", "per_thread"])
+def test_forced_variant_ragged_tiles_every_optimizer(variant, optkey):
+    """the staged kernel's SGD, AdamW and Test instantiations, and Adam / AdamW with a binding clip_gradient after a
+    rescale_grad != 1, on the ragged sizes above"""
+    _run_keyset(variant, optkey, 2, [4, 2052, 8196, 3 * 2048 + 12, (1 << 20) + 4, 12], steps=3, seed=5)
+
+
+def test_forced_staged_kernel_local_store_six_sources():
+    """kv.create('local'): CommCPU's groups of four (in0 += ((in1+in2)+in3)+in4) inside the staged kernel"""
+    _run_keyset("bulk", "adam", 6, [4, 2052, 8196, 100004], steps=2, seed=9, kvtype="local")
 
 
 # ---------------------------------------------------------------------------
