@@ -143,8 +143,8 @@ MXKV_DLL int MXKVStoreSendCommmandToServers(KVStoreHandle handle, int cmd_id, co
 /* ---- MXKVB200 extensions -------------------------------------------------- */
 /* Fused optimizer: what Python's Updater + sgd_update/adam_update ops do per key in the
  * reference (python/mxnet/optimizer/updater.py:39-93) happens inside the reduce kernel.
- * name: "sgd" | "nag" | "adam" | "adamw" | "test" | "lamb" | "lans" | "lars"; kwargs use the reference's
- * hyper-parameter names (learning_rate, wd, momentum, rescale_grad, clip_gradient, beta1, beta2,
+ * name: "sgd" | "nag" | "adam" | "adamw" | "adabelief" | "test" | "lamb" | "lans" | "lars"; kwargs use the
+ * reference's hyper-parameter names (learning_rate, wd, momentum, rescale_grad, clip_gradient, beta1, beta2,
  * epsilon, eta, multi_precision, lazy_update, correct_bias, lower_bound, upper_bound,
  * bias_correction).  lamb / lans / lars additionally take skip_nonfinite=True: when any merged
  * gradient of a push holds inf/nan, that push changes neither weights nor optimizer state (the AMP
@@ -158,8 +158,8 @@ MXKV_DLL int MXKVB200SetOptimizerMult(KVStoreHandle handle, int key, const char*
 /* The native counterpart of the reference's per-device Updater (python/mxnet/optimizer/updater.py:
  * 39-93) and of the multi-tensor update operators it ends in when parameters are NOT updated on the
  * kvstore (multi_sgd_update / multi_sgd_mom_update / multi_mp_sgd_*, src/operator/optimizer_op-inl.h:
- * 207-375; nag_mom_update / mp_nag_mom_update per weight, :1029-1092; multi_adamw, multi_lamb,
- * multi_lans).  Create the handle with MXKVStoreCreate("updater"), give it an optimizer with MXKVB200SetOptimizer, then every call updates all (weight, grad) pairs
+ * 207-375; nag_mom_update / mp_nag_mom_update per weight, :1029-1092; multi_adamw, multi_adabelief,
+ * multi_lamb, multi_lans).  Create the handle with MXKVStoreCreate("updater"), give it an optimizer with MXKVB200SetOptimizer, then every call updates all (weight, grad) pairs
  * IN PLACE with one launch (sequence) on their GPU.  Optimizer state of an index is created on first
  * sight and is reachable through MXKVB200GetState / SetState / Get|SetUpdateCount.  One handle serves
  * one device, like the reference's `Trainer._updaters[dev]`.  Never collective.  grads == NULL only
@@ -170,7 +170,8 @@ MXKV_DLL int MXKVB200UpdaterStepEx(KVStoreHandle handle, uint32_t num, const cha
                                    NDArrayHandle* weights, NDArrayHandle* grads);
 /* Introspection: the per-key scalars the fused kernel would receive for the key's CURRENT update count
  * (learning rate with lr_mult and, for Adam, the host-side bias correction folded in; weight decay with
- * wd_mult; AdamW: operator lr = 1 and eta = the bias-corrected learning rate).  Host-only, no GPU needed. */
+ * wd_mult; AdamW and AdaBelief: operator lr = 1 and eta = the bias-corrected learning rate).  Host-only,
+ * no GPU needed. */
 MXKV_DLL int MXKVB200GetKeyHyper(KVStoreHandle handle, int key, const char* str_key, float* lr, float* wd,
                                  float* eta);
 /* per-key switch of a fused optimizer.  "no_trust_ratio" != 0: LARS keeps the plain learning rate

@@ -100,16 +100,16 @@ __device__ __forceinline__ void process_packets(const TensorWork& tw, const int6
         pw.load(tw.w, e[u]);
         pw.unpack(w[u]);
       }
-      if (OPT == OPT_SGD_MOM || OPT == OPT_ADAM || OPT == OPT_ADAMW || OPT == OPT_ADAM_STD || OPT == OPT_NAG) ldf<N>(tw.s0, e[u], s0[u]);
-      if (OPT == OPT_ADAM || OPT == OPT_ADAMW || OPT == OPT_ADAM_STD) ldf<N>(tw.s1, e[u], s1[u]);
+      if (OptHasS0(OPT)) ldf<N>(tw.s0, e[u], s0[u]);
+      if (OptHasS1(OPT)) ldf<N>(tw.s1, e[u], s1[u]);
     }
 #pragma unroll
     for (int u = 0; u < U; ++u) {
       if (!ok[u]) continue;
 #pragma unroll
       for (int i = 0; i < N; ++i) wnew[u][i] = update_one<OPT>(acc[u][i], w[u][i], s0[u][i], s1[u][i], h);
-      if (OPT == OPT_SGD_MOM || OPT == OPT_ADAM || OPT == OPT_ADAMW || OPT == OPT_ADAM_STD || OPT == OPT_NAG) stf<N>(tw.s0, e[u], s0[u]);
-      if (OPT == OPT_ADAM || OPT == OPT_ADAMW || OPT == OPT_ADAM_STD) stf<N>(tw.s1, e[u], s1[u]);
+      if (OptHasS0(OPT)) stf<N>(tw.s0, e[u], s0[u]);
+      if (OptHasS1(OPT)) stf<N>(tw.s1, e[u], s1[u]);
       if (MP) stf<N>(tw.w32, e[u], wnew[u]);
     }
   }
@@ -251,8 +251,8 @@ kv_dense_bulk_kernel(DenseLaunch L) {
   const uint32_t arr_bytes = static_cast<uint32_t>(tile) * 4u;
   const uint32_t stage_bytes = arr_bytes * static_cast<uint32_t>(L.bulk_arrays);
   constexpr bool HAS_W = OPT != OPT_NONE;
-  constexpr bool HAS_S0 = OPT == OPT_SGD_MOM || OPT == OPT_ADAM || OPT == OPT_ADAMW || OPT == OPT_NAG;
-  constexpr bool HAS_S1 = OPT == OPT_ADAM || OPT == OPT_ADAMW;
+  constexpr bool HAS_S0 = OptHasS0(OPT);
+  constexpr bool HAS_S1 = OptHasS1(OPT);
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < stages; ++s) mbar_init(&full[s], 1);
@@ -418,6 +418,7 @@ static BulkKernelFn pick_bulk(int opt, int mp) {
     case OPT_ADAMW: return mp ? kv_dense_bulk_kernel<OPT_ADAMW, true> : kv_dense_bulk_kernel<OPT_ADAMW, false>;
     case OPT_TEST: return mp ? kv_dense_bulk_kernel<OPT_TEST, true> : kv_dense_bulk_kernel<OPT_TEST, false>;
     case OPT_NAG: return mp ? kv_dense_bulk_kernel<OPT_NAG, true> : kv_dense_bulk_kernel<OPT_NAG, false>;
+    case OPT_ADABELIEF: return mp ? kv_dense_bulk_kernel<OPT_ADABELIEF, true> : kv_dense_bulk_kernel<OPT_ADABELIEF, false>;
     default: return nullptr;
   }
 }
@@ -498,8 +499,8 @@ __global__ void __launch_bounds__(kThreads, (U >= 4 || PIPE) ? 1 : 2)
 kv_dense_nvls_kernel(DenseLaunch L) {
   __shared__ TensorWork tw;
   barrier_start(L.sync);
-  constexpr bool HAS_S0 = OPT == OPT_SGD_MOM || OPT == OPT_ADAM || OPT == OPT_ADAMW || OPT == OPT_NAG;
-  constexpr bool HAS_S1 = OPT == OPT_ADAM || OPT == OPT_ADAMW;
+  constexpr bool HAS_S0 = OptHasS0(OPT);
+  constexpr bool HAS_S1 = OptHasS1(OPT);
   int cur = -1;
   int64_t c = blockIdx.x;
   NvlsChunk k, kn;
@@ -586,14 +587,17 @@ static NvlsKernelFn pick_nvls_opt(int opt, int mp) {
     case OPT_ADAMW: return mp ? kv_dense_nvls_kernel<OPT_ADAMW, true, U, PIPE> : kv_dense_nvls_kernel<OPT_ADAMW, false, U, PIPE>;
     case OPT_TEST: return mp ? kv_dense_nvls_kernel<OPT_TEST, true, U, PIPE> : kv_dense_nvls_kernel<OPT_TEST, false, U, PIPE>;
     case OPT_NAG: return mp ? kv_dense_nvls_kernel<OPT_NAG, true, U, PIPE> : kv_dense_nvls_kernel<OPT_NAG, false, U, PIPE>;
+    case OPT_ADABELIEF:
+      return mp ? kv_dense_nvls_kernel<OPT_ADABELIEF, true, U, PIPE> : kv_dense_nvls_kernel<OPT_ADABELIEF, false, U, PIPE>;
     default: return nullptr;
   }
 }
 
 // the instantiated (U, PIPE) points; anything else is rounded down to the nearest one
-// (Adam / AdamW carry three state packets per gradient packet: 8 requests would spill at 128 registers)
+// (the kinds with two state arrays -- Adam, AdamW, AdaBelief -- carry three state packets per gradient packet:
+// 8 requests would spill at 128 registers)
 static int nvls_round_unroll(int unroll, int opt) {
-  if ((opt == OPT_ADAM || opt == OPT_ADAMW) && unroll > 4) unroll = 4;
+  if (OptHasS1(opt) && unroll > 4) unroll = 4;
   return unroll >= 8 ? 8 : (unroll >= 4 ? 4 : (unroll >= 2 ? 2 : 1));
 }
 
@@ -687,6 +691,7 @@ static DenseKernelFn pick_opt(int opt, bool mp, bool small_n, bool allow_non_mp)
       case OPT_ADAMW: return pick_n<T, OPT_ADAMW, true>(small_n);
       case OPT_TEST: return pick_n<T, OPT_TEST, true>(small_n);
       case OPT_NAG: return pick_n<T, OPT_NAG, true>(small_n);
+      case OPT_ADABELIEF: return pick_n<T, OPT_ADABELIEF, true>(small_n);
       default: return nullptr;
     }
   }
@@ -708,6 +713,7 @@ static DenseKernelFn pick_kernel(const DenseLaunch& L) {
         case OPT_ADAMW: return pick_n<float, OPT_ADAMW, false>(sn);
         case OPT_TEST: return pick_n<float, OPT_TEST, false>(sn);
         case OPT_NAG: return pick_n<float, OPT_NAG, false>(sn);
+        case OPT_ADABELIEF: return pick_n<float, OPT_ADABELIEF, false>(sn);
         case OPT_SGD_STD: return kv_dense_kernel<float, OPT_SGD_STD, false, false>;
         case OPT_ADAM_STD: return kv_dense_kernel<float, OPT_ADAM_STD, false, false>;
         default: return nullptr;

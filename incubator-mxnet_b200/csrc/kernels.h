@@ -40,9 +40,21 @@ enum OptKind : int {
   OPT_LAMB = 8,     // multi_lamb_update / multi_mp_lamb_update   contrib/multi_lamb.cc:36-120
   OPT_LANS = 9,     // multi_lans_update / multi_mp_lans_update   contrib/multi_lans.cc:36-130
   OPT_LARS = 10,    // LARS._get_lars + (mp_)sgd(_mom)_update     python/mxnet/optimizer/lars.py:117-133,244-275
-  OPT_NAG = 11      // NAGMomKernel / MP_NAGMomKernel        optimizer_op-inl.h:1029-1044,1066-1090
+  OPT_NAG = 11,     // NAGMomKernel / MP_NAGMomKernel        optimizer_op-inl.h:1029-1044,1066-1090
+  OPT_ADABELIEF = 12  // MultiMPAdaBeliefKernel              contrib/adabelief-inl.h:354-384
 };
 inline bool IsNormOpt(int kind) { return kind == OPT_LAMB || kind == OPT_LANS || kind == OPT_LARS; }
+
+// The fp32 state arrays an element-wise kind streams through update_one: s0 (momentum / mean), s1 (variance).
+// Every dense kernel loads and stores exactly these, and the staged kernel counts them among its staged arrays.
+// The layer-wise adaptive kinds keep their state rules with their launch sequence (KVStore::EnsureState).
+__host__ __device__ constexpr bool OptHasS0(int kind) {
+  return kind == OPT_SGD_MOM || kind == OPT_ADAM || kind == OPT_ADAMW || kind == OPT_ADAM_STD || kind == OPT_NAG ||
+         kind == OPT_ADABELIEF;
+}
+__host__ __device__ constexpr bool OptHasS1(int kind) {
+  return kind == OPT_ADAM || kind == OPT_ADAMW || kind == OPT_ADAM_STD || kind == OPT_ADABELIEF;
+}
 
 enum SumOrder : int {
   ORDER_DEVICE = 0,  // ((in0+in1)+in2)+...                  ndarray_function-inl.h:457-486

@@ -435,6 +435,7 @@ void KVStore::SetOptimizer(const std::string& name, const std::vector<std::pair<
   else if (n == "lans") { c.kind = OPT_LANS; c.lr = 0.001; c.eps = 1e-6f; }    // lans.py:61-63
   else if (n == "lars") { c.kind = OPT_LARS; c.lr = 0.1; }                     // lars.py:77-79
   else if (n == "nag") { c.kind = OPT_NAG; c.lr = 0.1; c.momentum = 0.9f; }     // nag.py:58
+  else if (n == "adabelief") { c.kind = OPT_ADABELIEF; c.lr = 0.001; c.eps = 1e-6f; }   // adabelief.py:79
   else MXKV_FATAL() << "optimizer '" << name << "' has no fused kernel; register a Python updater instead";
   for (auto& kv : kwargs) {
     const std::string& k = kv.first;
@@ -520,26 +521,29 @@ void KVStore::SetOptimizerMult(bool str_key, int ikey, const std::string& skey, 
   opt_.wd_mult[key] = wd_mult;
 }
 
-// AdamW: the reference's optimizer class hands the operator lr = 1 and eta = the (bias-corrected)
-// learning rate (`lrs=np.ones(...)`, `etas=lrs`, python/mxnet/optimizer/adamW.py:176-200), which is
-// how `w -= eta * (lr * m / (sqrt(v) + eps) + wd * w)` (contrib/adamw-inl.h:101-124) becomes the
-// documented `w -= lr * (m / (sqrt(v) + eps) + wd * w)`.  opt_.eta is an additional schedule multiplier
-// of this engine's own (1 by default; the reference class has none).
+// AdamW and AdaBelief: the reference's optimizer classes hand the operator lr = 1 and eta = the
+// (bias-corrected) learning rate (`lrs=np.ones(...)`, `etas=lrs`, python/mxnet/optimizer/adamW.py:176-200,
+// adabelief.py:171-220), which is how `w -= eta * (lr * m / (sqrt(v) + eps) + wd * w)`
+// (contrib/adamw-inl.h:101-124) becomes the documented `w -= lr * (m / (sqrt(v) + eps) + wd * w)`.
+// opt_.eta is an additional schedule multiplier of this engine's own (1 by default; the reference classes
+// have none).
+static bool EtaCarriesLR(int kind) { return kind == OPT_ADAMW || kind == OPT_ADABELIEF; }
+
 float KVStore::KeyLR(const KeyState& ks) const {
-  if (opt_.kind == OPT_ADAMW) return 1.0f;
+  if (EtaCarriesLR(opt_.kind)) return 1.0f;
   return static_cast<float>(KeyLRd(ks));
 }
 
-// `_adamw_update` and its multi / mp forms leave everything untouched when the rescale_grad scalar is
-// 0, inf or nan (contrib/adamw-inl.h:455: the AMP loss-scale path); Optimizer._update_count has already
-// run by then (adamW.py:158).
-bool KVStore::AdamWSkips() const {
-  return opt_.enabled && updater_ == nullptr && opt_.kind == OPT_ADAMW &&
+// `_adamw_update`, `_adabelief_update` and their multi / mp forms leave everything untouched when the
+// rescale_grad scalar is 0, inf or nan (contrib/adamw-inl.h:455, contrib/adabelief-inl.h:454-466: the AMP
+// loss-scale path); Optimizer._update_count has already run by then (adamW.py:158, adabelief.py:171).
+bool KVStore::SkipsOnRescale() const {
+  return opt_.enabled && updater_ == nullptr && EtaCarriesLR(opt_.kind) &&
          (!std::isfinite(opt_.rescale) || opt_.rescale == 0.f);
 }
 
 float KVStore::KeyEta(const KeyState& ks) const {
-  if (opt_.kind == OPT_ADAMW) return static_cast<float>(KeyLRd(ks) * opt_.eta_d);
+  if (EtaCarriesLR(opt_.kind)) return static_cast<float>(KeyLRd(ks) * opt_.eta_d);
   return opt_.eta;
 }
 
@@ -549,7 +553,8 @@ double KVStore::KeyLRd(const KeyState& ks) const {
   double lr = opt_.lr;
   auto it = opt_.lr_mult.find(ks.key);
   if (it != opt_.lr_mult.end()) lr *= it->second;
-  if (opt_.kind == OPT_ADAM || (opt_.kind == OPT_ADAMW && opt_.correct_bias)) {   // adamW.py:175-182
+  // adamW.py:175-182, adabelief.py:174-181
+  if (opt_.kind == OPT_ADAM || (EtaCarriesLR(opt_.kind) && opt_.correct_bias)) {
     const double t = static_cast<double>(ks.count);
     const double coef1 = 1. - std::pow(opt_.beta1, t);
     const double coef2 = 1. - std::pow(opt_.beta2, t);
@@ -650,10 +655,9 @@ void KVStore::EnsureState(KeyState& ks, Replica& r, bool mp) {
   const Context ctx{kGPU, r.dev};
   DeviceGuard g(r.dev);
   cudaStream_t s = rt->Dev(r.dev).stream;
-  const bool need_s0 = opt_.kind == OPT_SGD_MOM || opt_.kind == OPT_ADAM || opt_.kind == OPT_ADAMW ||
-                       opt_.kind == OPT_NAG || opt_.kind == OPT_LAMB || opt_.kind == OPT_LANS ||
+  const bool need_s0 = OptHasS0(opt_.kind) || opt_.kind == OPT_LAMB || opt_.kind == OPT_LANS ||
                        (opt_.kind == OPT_LARS && opt_.momentum != 0.f);      // lars.py:96-101
-  const bool need_s1 = opt_.kind == OPT_ADAM || opt_.kind == OPT_ADAMW || opt_.kind == OPT_LAMB || opt_.kind == OPT_LANS;
+  const bool need_s1 = OptHasS1(opt_.kind) || opt_.kind == OPT_LAMB || opt_.kind == OPT_LANS;
   if (IsNormOpt(opt_.kind)) {
     // temporaries between the phases and the per-key totals the peers read (allocated collectively
     // in one-process-per-GPU mode: every rank reaches this point for the same keys in the same order)
@@ -812,7 +816,7 @@ void KVStore::PushImpl(const std::vector<int>& keys, const std::vector<NDArray>&
       PushRowSparse(GetKey(uniq[i]), grouped[i]);
       continue;
     }
-    if (AdamWSkips()) { ks.count += 1; continue; }
+    if (SkipsOnRescale()) { ks.count += 1; continue; }
     // BASELINE configs[0], the reference's CPU-runnable case: ONE host-resident value pushed to a key that has
     // never met a GPU, nothing to run on it (no updater, no optimizer, no compression).  The reference does no
     // arithmetic here either -- Reduce hands a single value back as it is (comm.h:128-131) and the store copies it
@@ -916,7 +920,7 @@ void KVStore::PushPullImpl(const std::vector<int>& vkeys, const std::vector<int>
     PullImpl(okeys, outs, priority, true);
     return;
   }
-  if (AdamWSkips()) {
+  if (SkipsOnRescale()) {
     for (int key : vu) PeekKey(key).count += 1;
     PullImpl(okeys, outs, priority, true);
     return;
@@ -1455,7 +1459,7 @@ bool KVStore::TryReplayRaw(int kind, uint32_t vnum, const int* vkeys, NDArray* c
   raw_single_ = false;
   if (deferred_ || !pending_.empty()) return false;      // the call joins (or must follow) the deferred queue
   if (plan_mode_ == 0 || key_type_ == kStringKey || hier_ || updater_ != nullptr || gc_bits_ != 0 ||
-      (opt_.enabled && (IsNormOpt(opt_.kind) || AdamWSkips())))
+      (opt_.enabled && (IsNormOpt(opt_.kind) || SkipsOnRescale())))
     return false;
   std::vector<uint64_t>& sig = raw_sig_;
   sig.clear();
@@ -2130,10 +2134,7 @@ void KVStore::LaunchWorks(const LaunchClassKey& ck, std::vector<std::vector<Tens
     int max_src = 1;
     for (int p = my_first; p <= my_last; ++p)
       for (auto& t : per_part[p]) { ok = ok && (t.flags & kWorkStaged); max_src = std::max(max_src, t.n_src); }
-    const int extra = (opt_kind != OPT_NONE ? 1 : 0) +
-                      ((opt_kind == OPT_SGD_MOM || opt_kind == OPT_ADAM || opt_kind == OPT_ADAMW ||
-                        opt_kind == OPT_NAG) ? 1 : 0) +
-                      ((opt_kind == OPT_ADAM || opt_kind == OPT_ADAMW) ? 1 : 0);
+    const int extra = (opt_kind != OPT_NONE ? 1 : 0) + (OptHasS0(opt_kind) ? 1 : 0) + (OptHasS1(opt_kind) ? 1 : 0);
     // the staged variant is taken (a) whenever sources are read over NVLink (more bytes in flight
     // against a ~2 us round trip) and (b) locally when a thread of the per-thread variant would have
     // few loads in flight (<= 2 sources, >= 3 streams).  With >= 3 local sources the per-thread variant
@@ -2459,7 +2460,7 @@ void KVStore::UpdaterStep(bool str_keys, const std::vector<int>& ikeys, const st
     r->fresh = true;
     ks.local_world = 0;
     if (bind_only) continue;
-    if (AdamWSkips()) { ks.count += 1; continue; }
+    if (SkipsOnRescale()) { ks.count += 1; continue; }
     if (grads[i].stype() == kRowSparseStorage) { sparse.emplace_back(key, grads[i]); continue; }
     Group grp;
     grp.key = key;

@@ -40,7 +40,7 @@ struct OptimizerConfig {
   float rescale = 1.f, clip = -1.f;
   bool multi_precision = false;
   bool lazy_update = false;   // row_sparse gradients: touch only the rows present (sgd.py:78, adam.py:77 default False)
-  bool correct_bias = true;   // AdamW only (python/mxnet/optimizer/adamW.py:80-88)
+  bool correct_bias = true;   // AdamW, AdaBelief (python/mxnet/optimizer/adamW.py:80-88, adabelief.py:79-87)
   // LAMB / LANS / LARS (python/mxnet/optimizer/{lamb,lans,lars}.py)
   float lower_bound = -1.f, upper_bound = -1.f;   // bounds on the weight norm, < 0: not set
   bool bias_correction = true;                     // LAMB
@@ -253,7 +253,7 @@ class KVStore {
   double KeyLRd(const KeyState& ks) const;
   float KeyLR(const KeyState& ks) const;
   float KeyEta(const KeyState& ks) const;
-  bool AdamWSkips() const;
+  bool SkipsOnRescale() const;
   float KeyWD(const KeyState& ks) const;
 
   // ---- multi-node ('dist_device_sync' over a configured Hierarchy, runtime.h) --------------------------

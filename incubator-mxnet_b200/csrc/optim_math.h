@@ -97,6 +97,17 @@ MXKV_HD float update_one(float g, float w, float& s0, float& s1, const Hyper& h)
     // NAGMomKernel: (w + momentum*mom) - lr*r;  MP_NAGMomKernel: w + (momentum*mom - lr*r)
     if (h.mp) return __fadd_rn(w, __fsub_rn(__fmul_rn(h.momentum, m), __fmul_rn(h.lr, r)));
     return __fsub_rn(__fadd_rn(w, __fmul_rn(h.momentum, m)), __fmul_rn(h.lr, r));
+  } else if (OPT == OPT_ADABELIEF) {
+    // MultiMPAdaBeliefKernel: wd is added BEFORE the clip; eps is added to the variance state every step
+    float r = __fmul_rn(h.rescale, g);
+    r = __fadd_rn(r, __fmul_rn(h.wd, w));
+    if (h.clip >= 0.0f) r = clipf(r, h.clip);
+    const float m = __fadd_rn(__fmul_rn(h.beta1, __fsub_rn(s0, r)), r);
+    const float d = __fsub_rn(m, r);
+    const float adj = __fmul_rn(d, d);
+    const float v = __fadd_rn(__fadd_rn(__fmul_rn(h.beta2, __fsub_rn(s1, adj)), adj), h.eps);
+    s0 = m; s1 = v;
+    return __fsub_rn(w, __fmul_rn(h.eta, __fdiv_rn(__fmul_rn(h.lr, m), __fadd_rn(__fsqrt_rn(v), h.eps))));
   }
   return g;  // OPT_NONE
 }

@@ -63,8 +63,8 @@ __device__ __forceinline__ void tree_packet(const TensorWork& tw, int64_t e, con
 #pragma unroll
     for (int i = 0; i < N; ++i) wnew[i] = acc[i];
   } else {
-    constexpr bool HAS_S0 = OPT == OPT_SGD_MOM || OPT == OPT_ADAM || OPT == OPT_ADAMW || OPT == OPT_NAG;
-    constexpr bool HAS_S1 = OPT == OPT_ADAM || OPT == OPT_ADAMW;
+    constexpr bool HAS_S0 = OptHasS0(OPT);
+    constexpr bool HAS_S1 = OptHasS1(OPT);
     float w[N], s0[N], s1[N];
     if (MP) {
       ldf<N>(tw.w32, e, w);
@@ -186,6 +186,7 @@ static TreeKernelFn pick_tree_opt(int opt, bool mp, bool allow_non_mp) {
       case OPT_ADAMW: return kv_dense_tree_kernel<T, OPT_ADAMW, true>;
       case OPT_TEST: return kv_dense_tree_kernel<T, OPT_TEST, true>;
       case OPT_NAG: return kv_dense_tree_kernel<T, OPT_NAG, true>;
+      case OPT_ADABELIEF: return kv_dense_tree_kernel<T, OPT_ADABELIEF, true>;
       default: return nullptr;
     }
   }
@@ -198,6 +199,7 @@ static TreeKernelFn pick_tree_opt(int opt, bool mp, bool allow_non_mp) {
       case OPT_ADAMW: return kv_dense_tree_kernel<T, OPT_ADAMW, false>;
       case OPT_TEST: return kv_dense_tree_kernel<T, OPT_TEST, false>;
       case OPT_NAG: return kv_dense_tree_kernel<T, OPT_NAG, false>;
+      case OPT_ADABELIEF: return kv_dense_tree_kernel<T, OPT_ADABELIEF, false>;
       default: return nullptr;
     }
   }

@@ -1,8 +1,8 @@
-"""Optimizer descriptors mirroring python/mxnet/optimizer/{optimizer,sgd,adam,adamW,updater}.py.
+"""Optimizer descriptors mirroring python/mxnet/optimizer/{optimizer,sgd,nag,adam,adamW,adabelief,updater}.py.
 
 Two roles:
 * describe the hyper-parameters of the optimizers that have a fused kernel in the native
-  engine (SGD / SGD-momentum / multi-precision SGD, NAG, Adam, AdamW, Test, and the layer-wise adaptive
+  engine (SGD / SGD-momentum / multi-precision SGD, NAG, Adam, AdamW, AdaBelief, Test, and the layer-wise adaptive
   LAMB / LANS / LARS) -- ``KVStore.set_optimizer``
   hands them to ``MXKVB200SetOptimizer`` and the update then runs inside the reduce kernel;
 * provide the generic ``Updater`` callback (updater.py:39-93) for any other Optimizer object:
@@ -336,6 +336,54 @@ class AdamW(Optimizer):
         return kw
 
 
+@register
+class AdaBelief(Optimizer):
+    """python/mxnet/optimizer/adabelief.py; fused kernels multi_adabelief_update / multi_mp_adabelief_update
+    (src/operator/contrib/adabelief-inl.h:354-384), driven like AdamW: operator ``lr = 1``, operator
+    ``eta = lr_t`` (adabelief.py:171-220), and a ``rescale_grad`` of 0 / inf / nan skips the update::
+
+        grad = clip(grad * rescale_grad + wd * weight, clip_gradient)
+        mean = beta1 * mean + (1 - beta1) * grad
+        var = beta2 * var + (1 - beta2) * (grad - mean)**2 + epsilon
+        lr_t = learning_rate * sqrt(1 - beta2**t) / (1 - beta1**t)      (correct_bias; else learning_rate)
+        weight = weight - lr_t * mean / (sqrt(var) + epsilon)
+    """
+    fused_name = "adabelief"
+
+    def __init__(self, learning_rate=0.001, beta1=0.9, beta2=0.999, epsilon=1e-6, correct_bias=True, **kwargs):
+        super(AdaBelief, self).__init__(learning_rate=learning_rate, **kwargs)
+        self.beta1, self.beta2, self.epsilon = beta1, beta2, epsilon
+        self.correct_bias = correct_bias
+
+    def fused_kwargs(self):
+        kw = super(AdaBelief, self).fused_kwargs()
+        kw.update(beta1=self.beta1, beta2=self.beta2, epsilon=self.epsilon, correct_bias=bool(self.correct_bias))
+        return kw
+
+    def create_state(self, index, weight):
+        import torch
+        w = weight.as_torch()
+        return (torch.zeros_like(w, dtype=torch.float32), torch.zeros_like(w, dtype=torch.float32))   # mean, var
+
+    def step(self, indices, weights, grads, states):     # adabelief.py:112-139
+        import torch
+        for index, weight, grad, state in zip(indices, weights, grads, states):
+            self._update_count(index)
+            lr = self._get_lr(index)
+            t = self._index_update_count[index]
+            w, g = weight.as_torch(), grad.as_torch()
+            # weight decay BEFORE the clip (unlike _prep_grad's order)
+            g = g.to(torch.float32) * self.rescale_grad + self._get_wd(index) * w
+            if self.clip_gradient is not None:
+                g = torch.clamp(g, -self.clip_gradient, self.clip_gradient)
+            if self.correct_bias:
+                lr *= math.sqrt(1. - self.beta2 ** t) / (1. - self.beta1 ** t)
+            mean, var = state
+            mean.mul_(self.beta1).add_((1. - self.beta1) * g)
+            var.mul_(self.beta2).add_((1. - self.beta2) * torch.square(g - mean)).add_(self.epsilon)
+            w.sub_(lr * (mean / (torch.sqrt(var) + self.epsilon)))
+
+
 class _LayerwiseAdaptive(Optimizer):
     """Shared part of LAMB / LANS / LARS: ``skip_nonfinite=True`` asks the store to leave weights and
     state alone when a merged gradient holds inf/nan (the AMP overflow skip, gluon/trainer.py:445-448,
@@ -536,7 +584,7 @@ class NativeUpdater(object):
     """Same call contract as :class:`Updater` (updater.py:39-93; ``index`` / ``grad`` / ``weight`` may be
     lists), but the whole list is updated IN PLACE by one fused launch (sequence) of the native engine
     -- what the reference does with ``multi_sgd_mom_update`` / ``multi_mp_sgd_*`` / ``multi_adamw`` /
-    ``multi_lamb`` / ``multi_lans`` when parameters are not updated on the kvstore (sgd.py:170-213,
+    ``multi_adabelief`` / ``multi_lamb`` / ``multi_lans`` when parameters are not updated on the kvstore (sgd.py:170-213,
     lamb.py:170-215).  One instance serves one device, like ``Trainer._updaters[dev]``."""
 
     def __init__(self, optimizer):

@@ -1,5 +1,7 @@
 """Step time of the fused NAG against fused SGD-momentum at N = 1 (one GPU, one gradient per key), and of NAG through
-the Python `step` (use_fused_step=False, the only way to run NAG before the fused kernel existed).
+the Python `step` (use_fused_step=False, the only way to run NAG before the fused kernel existed).  With
+`--pair adabelief`: the fused AdaBelief against the fused Adam instead (both read g, w, mean, var and write stored w,
+mean, var, out: 32 bytes per float32 element).
 
 Two key sets: the bench sweep (9 float32 keys, 2^10 ... 2^26 elements) and ResNet-50's 193 gradient-carrying arrays
 (bench.py: keyset).  Both fused optimizers move the same bytes per element (read g, w, mom; write stored w, mom, out),
@@ -8,7 +10,7 @@ engine's stream (the Python path: host clock around a device synchronise, its to
 dense kernel variant that ran (launch counters), and one step checked against the CPU oracle.  The card's name and
 power limit are read with nvidia-smi in the same call and printed with the numbers.
 
-    python tools/optimizer_rate.py [--steps 200] [--warmup 20] [--rounds 3]
+    python tools/optimizer_rate.py [--pair nag|adabelief] [--steps 200] [--warmup 20] [--rounds 3]
 """
 import argparse
 import ctypes
@@ -28,6 +30,10 @@ from bench import keyset, nelem, tile_fill  # noqa: E402
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 KW = dict(learning_rate=0.01, momentum=0.9, wd=1e-4)
+KW_ADAPTIVE = dict(learning_rate=0.001, wd=1e-4)
+# --pair: (baseline, optimizer under test); the python step is timed for the NAG pair only
+PAIRS = {"nag": ("sgd", "nag"), "adabelief": ("adam", "adabelief")}
+LABELS = {"sgd": "sgd_momentum", "nag": "nag", "adam": "adam", "adabelief": "adabelief"}
 VARIANTS = ("per_thread", "bulk", "nvls", "tree")
 
 
@@ -54,10 +60,10 @@ class Case(object):
         self.grads_np = [tile_fill(np.random.default_rng(1234 + k), -1, 1, s) for k, s in enumerate(shapes)]
         self.kv = mx.kv.create("device")
         self.kv.init(self.keys, [mx.nd.array(w, mx.gpu(0)) for w in w0])
-        if optname == "sgd":
-            opt = mx.optimizer.SGD(**KW)
-        else:
-            opt = mx.optimizer.NAG(**dict(KW, **({} if fused else {"use_fused_step": False})))
+        self.kw = KW if optname in ("sgd", "nag") else KW_ADAPTIVE
+        cls = {"sgd": mx.optimizer.SGD, "nag": mx.optimizer.NAG, "adam": mx.optimizer.Adam,
+               "adabelief": mx.optimizer.AdaBelief}[optname]
+        opt = cls(**dict(self.kw, **({} if fused else {"use_fused_step": False})))
         self.kv.set_optimizer(opt)
         self.grads = [mx.nd.array(g, mx.gpu(0)) for g in self.grads_np]
         self.outs = [mx.nd.empty(s, mx.gpu(0)) for s in shapes]
@@ -73,8 +79,14 @@ class Case(object):
         self.mx.nd.waitall()
         import torch
         torch.cuda.synchronize()
-        import nag_oracle as N
-        oopt = N.OracleNAG(**KW) if self.optname == "nag" else O.OracleOptimizer(self.optname, **KW)
+        if self.optname == "nag":
+            import nag_oracle as N
+            oopt = N.OracleNAG(**self.kw)
+        elif self.optname == "adabelief":
+            import adabelief_oracle as A
+            oopt = A.OracleAdaBelief(**self.kw)
+        else:
+            oopt = O.OracleOptimizer(self.optname, **self.kw)
         exact, close = True, True
         for k in self.keys:
             w = self.w0[k].reshape(-1).copy()
@@ -113,6 +125,7 @@ def time_case(mx, torch, stream, case, steps, warmup):
 
 def main():
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
+    ap.add_argument("--pair", choices=sorted(PAIRS), default="nag")
     ap.add_argument("--steps", type=int, default=200)
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--rounds", type=int, default=3)
@@ -123,10 +136,12 @@ def main():
     import mxnet_b200 as mx
     info = card()
     stream = engine_stream(mx, torch)
-    result = {"card": info, "steps": args.steps, "warmup": args.warmup, "rounds": args.rounds, "cases": []}
+    result = {"card": info, "pair": args.pair, "steps": args.steps, "warmup": args.warmup, "rounds": args.rounds,
+              "cases": []}
+    base, test = PAIRS[args.pair]
     for ksname in ("sweep", "resnet50"):
         shapes = keyset(ksname)
-        cases = [("sgd", True), ("nag", True)] + ([("nag", False)] if ksname == "resnet50" else [])
+        cases = [(base, True), (test, True)] + ([(test, False)] if ksname == "resnet50" and test == "nag" else [])
         built = {c: Case(mx, shapes, c[0], c[1]) for c in cases}
         checks = {c: built[c].check() for c in cases}
         times = {c: [] for c in cases}
@@ -137,7 +152,7 @@ def main():
                 times[c].append(ms)
         for c in cases:
             ent = {"keyset": ksname, "keys": len(shapes), "elements": int(sum(nelem(s) for s in shapes)),
-                   "optimizer": ("nag" if c[0] == "nag" else "sgd_momentum") + ("" if c[1] else " (python step)"),
+                   "optimizer": LABELS[c[0]] + ("" if c[1] else " (python step)"),
                    "ms_per_step": times[c], "ms_median": float(np.median(times[c])), "variant": variants[c],
                    "oracle_check": checks[c]}
             result["cases"].append(ent)
