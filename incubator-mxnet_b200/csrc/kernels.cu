@@ -89,7 +89,7 @@ __device__ __forceinline__ void process_packets(const TensorWork& tw, const int6
 #pragma unroll
       for (int i = 0; i < N; ++i) wnew[u][i] = acc[u][i];
   } else {
-    float w[U][N], s0[U][N], s1[U][N];
+    float w[U][N], s0[U][N], s1[U][N], s2[U][N];
 #pragma unroll
     for (int u = 0; u < U; ++u) {
       if (!ok[u]) continue;
@@ -102,14 +102,16 @@ __device__ __forceinline__ void process_packets(const TensorWork& tw, const int6
       }
       if (OptHasS0(OPT)) ldf<N>(tw.s0, e[u], s0[u]);
       if (OptHasS1(OPT)) ldf<N>(tw.s1, e[u], s1[u]);
+      if (OptHasS2(OPT)) ldf<N>(tw.s2, e[u], s2[u]);
     }
 #pragma unroll
     for (int u = 0; u < U; ++u) {
       if (!ok[u]) continue;
 #pragma unroll
-      for (int i = 0; i < N; ++i) wnew[u][i] = update_one<OPT>(acc[u][i], w[u][i], s0[u][i], s1[u][i], h);
+      for (int i = 0; i < N; ++i) wnew[u][i] = update_one<OPT>(acc[u][i], w[u][i], s0[u][i], s1[u][i], s2[u][i], h);
       if (OptHasS0(OPT)) stf<N>(tw.s0, e[u], s0[u]);
       if (OptHasS1(OPT)) stf<N>(tw.s1, e[u], s1[u]);
+      if (OptHasS2(OPT)) stf<N>(tw.s2, e[u], s2[u]);
       if (MP) stf<N>(tw.w32, e[u], wnew[u]);
     }
   }
@@ -130,7 +132,9 @@ kv_dense_kernel(DenseLaunch L) {
 
   // 16-bit gradients with fp32 master/state: 4-element packets (8 B of gradient against
   // 16 B of every fp32 stream) keep the kernel inside 64 registers.
-  constexpr int NV = (OPT != OPT_NONE && sizeof(T) == 2) ? 4 : 16 / sizeof(T);
+  // Float32 keys of a kind with three state arrays (centered RMSProp) take one element per step: a 4-element packet
+  // of each of the five fp32 streams next to a batch of 16-byte source loads spills at 64 registers.
+  constexpr int NV = (OPT != OPT_NONE && sizeof(T) == 2) ? 4 : (OptHasS2(OPT) ? 1 : 16 / sizeof(T));
   constexpr int BATCH = SMALLN ? 2 : 4;
   constexpr int U = SMALLN ? 2 : 1;
   const bool native_half_add = (sizeof(T) == 2) && !L.fp32_accum && (OPT == OPT_NONE);
@@ -155,6 +159,7 @@ kv_dense_kernel(DenseLaunch L) {
     h.lr = tw.lr; h.wd = tw.wd; h.eta = tw.eta;
     h.rescale = L.rescale; h.clip = L.clip; h.momentum = L.momentum;
     h.beta1 = L.beta1; h.beta2 = L.beta2; h.eps = L.eps;
+    h.rho = L.rho; h.clip_weights = L.clip_weights;
     h.mp = sizeof(T) == 2 && L.mp_arith != 0;
 
     const int64_t cb = tw.begin + (c - L.chunk_prefix[lo]) * L.chunk_elems;
@@ -253,6 +258,7 @@ kv_dense_bulk_kernel(DenseLaunch L) {
   constexpr bool HAS_W = OPT != OPT_NONE;
   constexpr bool HAS_S0 = OptHasS0(OPT);
   constexpr bool HAS_S1 = OptHasS1(OPT);
+  constexpr bool HAS_S2 = OptHasS2(OPT);
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < stages; ++s) mbar_init(&full[s], 1);
@@ -265,7 +271,7 @@ kv_dense_bulk_kernel(DenseLaunch L) {
 
   // tiles of this block: groups of G consecutive tiles, block-cyclic -- tile(i) = ((i / G) * grid + block) * G + i % G.
   // G = 1 is the plain strided walk: all blocks stream through one narrow window of every array (best for DRAM on
-  // large keys) but every block meets every key of the work list and reloads a 400-byte descriptor each time, which
+  // large keys) but every block meets every key of the work list and reloads a 416-byte descriptor each time, which
   // costs a large share of the kernel on a model of hundreds of small keys (BERT-base).  A contiguous range per
   // block has the opposite profile.  Small groups keep the window narrow and divide the descriptor switches by G
   // (MXKV_B200_BULK_GROUP); the host groups only work lists of many keys (kvstore.cc: LaunchWorks) and keeps G = 1
@@ -304,7 +310,7 @@ kv_dense_bulk_kernel(DenseLaunch L) {
     const int64_t ce = (cb + tile < w->end) ? cb + tile : w->end;
     const uint32_t bytes = static_cast<uint32_t>(ce - cb) * 4u;
     const int n = w->n_src;
-    const int narr = n + (HAS_W ? 1 : 0) + (HAS_S0 ? 1 : 0) + (HAS_S1 ? 1 : 0);
+    const int narr = n + (HAS_W ? 1 : 0) + (HAS_S0 ? 1 : 0) + (HAS_S1 ? 1 : 0) + (HAS_S2 ? 1 : 0);
     const int s = static_cast<int>(i % stages);
     unsigned char* base = bulk_smem + static_cast<size_t>(s) * stage_bytes;
     mbar_expect_tx(&full[s], bytes * static_cast<uint32_t>(narr));
@@ -317,6 +323,7 @@ kv_dense_bulk_kernel(DenseLaunch L) {
     }
     if (HAS_S0) { bulk_g2s(base + static_cast<size_t>(a) * arr_bytes, w->s0 + cb, bytes, &full[s]); ++a; }
     if (HAS_S1) { bulk_g2s(base + static_cast<size_t>(a) * arr_bytes, w->s1 + cb, bytes, &full[s]); ++a; }
+    if (HAS_S2) { bulk_g2s(base + static_cast<size_t>(a) * arr_bytes, w->s2 + cb, bytes, &full[s]); ++a; }
   };
 
   if (threadIdx.x == 0) {
@@ -343,6 +350,7 @@ kv_dense_bulk_kernel(DenseLaunch L) {
     h.lr = tw.lr; h.wd = tw.wd; h.eta = tw.eta;
     h.rescale = L.rescale; h.clip = L.clip; h.momentum = L.momentum;
     h.beta1 = L.beta1; h.beta2 = L.beta2; h.eps = L.eps;
+    h.rho = L.rho; h.clip_weights = L.clip_weights;
     h.mp = false;                     // float32 keys only
     const int64_t cb = tw.begin + (c - L.chunk_prefix[lo]) * tile;
     const int64_t ce = (cb + tile < tw.end) ? cb + tile : tw.end;
@@ -383,7 +391,7 @@ kv_dense_bulk_kernel(DenseLaunch L) {
         int a = n;
         const float4 w4 = reinterpret_cast<const float4*>(base + static_cast<size_t>(a) * arr_bytes)[v]; ++a;
         float w[4] = {w4.x, w4.y, w4.z, w4.w};
-        float s0[4] = {0.f, 0.f, 0.f, 0.f}, s1[4] = {0.f, 0.f, 0.f, 0.f};
+        float s0[4] = {0.f, 0.f, 0.f, 0.f}, s1[4] = {0.f, 0.f, 0.f, 0.f}, s2[4] = {0.f, 0.f, 0.f, 0.f};
         if (HAS_S0) {
           const float4 t4 = reinterpret_cast<const float4*>(base + static_cast<size_t>(a) * arr_bytes)[v]; ++a;
           s0[0] = t4.x; s0[1] = t4.y; s0[2] = t4.z; s0[3] = t4.w;
@@ -392,10 +400,15 @@ kv_dense_bulk_kernel(DenseLaunch L) {
           const float4 t4 = reinterpret_cast<const float4*>(base + static_cast<size_t>(a) * arr_bytes)[v]; ++a;
           s1[0] = t4.x; s1[1] = t4.y; s1[2] = t4.z; s1[3] = t4.w;
         }
+        if (HAS_S2) {
+          const float4 t4 = reinterpret_cast<const float4*>(base + static_cast<size_t>(a) * arr_bytes)[v]; ++a;
+          s2[0] = t4.x; s2[1] = t4.y; s2[2] = t4.z; s2[3] = t4.w;
+        }
 #pragma unroll
-        for (int j = 0; j < 4; ++j) wnew[j] = update_one<OPT>(acc[j], w[j], s0[j], s1[j], h);
+        for (int j = 0; j < 4; ++j) wnew[j] = update_one<OPT>(acc[j], w[j], s0[j], s1[j], s2[j], h);
         if (HAS_S0) stf<4>(tw.s0, e, s0);
         if (HAS_S1) stf<4>(tw.s1, e, s1);
+        if (HAS_S2) stf<4>(tw.s2, e, s2);
         if (MP) stf<4>(tw.w32, e, wnew);
       }
       const int m = tw.n_out;
@@ -419,6 +432,9 @@ static BulkKernelFn pick_bulk(int opt, int mp) {
     case OPT_TEST: return mp ? kv_dense_bulk_kernel<OPT_TEST, true> : kv_dense_bulk_kernel<OPT_TEST, false>;
     case OPT_NAG: return mp ? kv_dense_bulk_kernel<OPT_NAG, true> : kv_dense_bulk_kernel<OPT_NAG, false>;
     case OPT_ADABELIEF: return mp ? kv_dense_bulk_kernel<OPT_ADABELIEF, true> : kv_dense_bulk_kernel<OPT_ADABELIEF, false>;
+    case OPT_RMSPROP: return mp ? kv_dense_bulk_kernel<OPT_RMSPROP, true> : kv_dense_bulk_kernel<OPT_RMSPROP, false>;
+    case OPT_RMSPROP_CENTERED:
+      return mp ? kv_dense_bulk_kernel<OPT_RMSPROP_CENTERED, true> : kv_dense_bulk_kernel<OPT_RMSPROP_CENTERED, false>;
     default: return nullptr;
   }
 }
@@ -501,6 +517,7 @@ kv_dense_nvls_kernel(DenseLaunch L) {
   barrier_start(L.sync);
   constexpr bool HAS_S0 = OptHasS0(OPT);
   constexpr bool HAS_S1 = OptHasS1(OPT);
+  constexpr bool HAS_S2 = OptHasS2(OPT);
   int cur = -1;
   int64_t c = blockIdx.x;
   NvlsChunk k, kn;
@@ -528,11 +545,12 @@ kv_dense_nvls_kernel(DenseLaunch L) {
     h.lr = tw.lr; h.wd = tw.wd; h.eta = tw.eta;
     h.rescale = L.rescale; h.clip = L.clip; h.momentum = L.momentum;
     h.beta1 = L.beta1; h.beta2 = L.beta2; h.eps = L.eps;
+    h.rho = L.rho; h.clip_weights = L.clip_weights;
     h.mp = false;                     // float32 keys only
     const int64_t nvec = (k.ce - k.cb) >> 2;
     const int n_plain = tw.n_out - tw.n_mc;
     // state of all U packets first (independent HBM loads in flight together), then the arithmetic
-    float w[U][4], s0[U][4], s1[U][4];
+    float w[U][4], s0[U][4], s1[U][4], s2[U][4];
     if (OPT != OPT_NONE) {
 #pragma unroll
       for (int u = 0; u < U; ++u) {
@@ -542,6 +560,7 @@ kv_dense_nvls_kernel(DenseLaunch L) {
         ldf<4>(MP ? tw.w32 : static_cast<const float*>(tw.w), e, w[u]);
         if (HAS_S0) ldf<4>(tw.s0, e, s0[u]);
         if (HAS_S1) ldf<4>(tw.s1, e, s1[u]);
+        if (HAS_S2) ldf<4>(tw.s2, e, s2[u]);
       }
     }
 #pragma unroll
@@ -556,9 +575,10 @@ kv_dense_nvls_kernel(DenseLaunch L) {
         for (int j = 0; j < 4; ++j) wnew[j] = acc[j];
       } else {
 #pragma unroll
-        for (int j = 0; j < 4; ++j) wnew[j] = update_one<OPT>(acc[j], w[u][j], s0[u][j], s1[u][j], h);
+        for (int j = 0; j < 4; ++j) wnew[j] = update_one<OPT>(acc[j], w[u][j], s0[u][j], s1[u][j], s2[u][j], h);
         if (HAS_S0) stf<4>(tw.s0, e, s0[u]);
         if (HAS_S1) stf<4>(tw.s1, e, s1[u]);
+        if (HAS_S2) stf<4>(tw.s2, e, s2[u]);
         if (MP) stf<4>(tw.w32, e, wnew);
       }
       for (int j = 0; j < n_plain; ++j) stf<4>(static_cast<float*>(tw.out[j]), e, wnew);
@@ -589,14 +609,24 @@ static NvlsKernelFn pick_nvls_opt(int opt, int mp) {
     case OPT_NAG: return mp ? kv_dense_nvls_kernel<OPT_NAG, true, U, PIPE> : kv_dense_nvls_kernel<OPT_NAG, false, U, PIPE>;
     case OPT_ADABELIEF:
       return mp ? kv_dense_nvls_kernel<OPT_ADABELIEF, true, U, PIPE> : kv_dense_nvls_kernel<OPT_ADABELIEF, false, U, PIPE>;
+    case OPT_RMSPROP:
+      return mp ? kv_dense_nvls_kernel<OPT_RMSPROP, true, U, PIPE> : kv_dense_nvls_kernel<OPT_RMSPROP, false, U, PIPE>;
+    case OPT_RMSPROP_CENTERED:
+      return mp ? kv_dense_nvls_kernel<OPT_RMSPROP_CENTERED, true, U, PIPE>
+                : kv_dense_nvls_kernel<OPT_RMSPROP_CENTERED, false, U, PIPE>;
     default: return nullptr;
   }
 }
 
+// Centered RMSProp (four state packets per gradient packet) at the default point U = 2 spills 120 / 96 bytes
+// (ptxas -v, 64 registers); at U = 1 it fits without spilling.
+constexpr int kNvlsMaxUnrollS2 = 1;
+
 // the instantiated (U, PIPE) points; anything else is rounded down to the nearest one
 // (the kinds with two state arrays -- Adam, AdamW, AdaBelief -- carry three state packets per gradient packet:
-// 8 requests would spill at 128 registers)
+// 8 requests would spill at 128 registers; centered RMSProp carries four: see kNvlsMaxUnrollS2)
 static int nvls_round_unroll(int unroll, int opt) {
+  if (OptHasS2(opt) && unroll > kNvlsMaxUnrollS2) unroll = kNvlsMaxUnrollS2;
   if (OptHasS1(opt) && unroll > 4) unroll = 4;
   return unroll >= 8 ? 8 : (unroll >= 4 ? 4 : (unroll >= 2 ? 2 : 1));
 }
@@ -692,6 +722,8 @@ static DenseKernelFn pick_opt(int opt, bool mp, bool small_n, bool allow_non_mp)
       case OPT_TEST: return pick_n<T, OPT_TEST, true>(small_n);
       case OPT_NAG: return pick_n<T, OPT_NAG, true>(small_n);
       case OPT_ADABELIEF: return pick_n<T, OPT_ADABELIEF, true>(small_n);
+      case OPT_RMSPROP: return pick_n<T, OPT_RMSPROP, true>(small_n);
+      case OPT_RMSPROP_CENTERED: return pick_n<T, OPT_RMSPROP_CENTERED, true>(small_n);
       default: return nullptr;
     }
   }
@@ -714,6 +746,8 @@ static DenseKernelFn pick_kernel(const DenseLaunch& L) {
         case OPT_TEST: return pick_n<float, OPT_TEST, false>(sn);
         case OPT_NAG: return pick_n<float, OPT_NAG, false>(sn);
         case OPT_ADABELIEF: return pick_n<float, OPT_ADABELIEF, false>(sn);
+        case OPT_RMSPROP: return pick_n<float, OPT_RMSPROP, false>(sn);
+        case OPT_RMSPROP_CENTERED: return pick_n<float, OPT_RMSPROP_CENTERED, false>(sn);
         case OPT_SGD_STD: return kv_dense_kernel<float, OPT_SGD_STD, false, false>;
         case OPT_ADAM_STD: return kv_dense_kernel<float, OPT_ADAM_STD, false, false>;
         default: return nullptr;

@@ -41,20 +41,26 @@ enum OptKind : int {
   OPT_LANS = 9,     // multi_lans_update / multi_mp_lans_update   contrib/multi_lans.cc:36-130
   OPT_LARS = 10,    // LARS._get_lars + (mp_)sgd(_mom)_update     python/mxnet/optimizer/lars.py:117-133,244-275
   OPT_NAG = 11,     // NAGMomKernel / MP_NAGMomKernel        optimizer_op-inl.h:1029-1044,1066-1090
-  OPT_ADABELIEF = 12  // MultiMPAdaBeliefKernel              contrib/adabelief-inl.h:354-384
+  OPT_ADABELIEF = 12, // MultiMPAdaBeliefKernel              contrib/adabelief-inl.h:354-384
+  OPT_RMSPROP = 13,   // RMSPropUpdateKernel                 optimizer_op-inl.h:2005-2031
+  OPT_RMSPROP_CENTERED = 14  // RMSPropAlexUpdateKernel      optimizer_op-inl.h:1905-1939
 };
 inline bool IsNormOpt(int kind) { return kind == OPT_LAMB || kind == OPT_LANS || kind == OPT_LARS; }
 
-// The fp32 state arrays an element-wise kind streams through update_one: s0 (momentum / mean), s1 (variance).
-// Every dense kernel loads and stores exactly these, and the staged kernel counts them among its staged arrays.
-// The layer-wise adaptive kinds keep their state rules with their launch sequence (KVStore::EnsureState).
+// The fp32 state arrays an element-wise kind streams through update_one: s0 (momentum / mean / RMSProp var;
+// centered RMSProp: mean), s1 (variance), s2 (centered RMSProp: momentum) -- the tuple order of the reference's
+// create_state.  Every dense kernel loads and stores exactly these, and the staged kernel counts them among its
+// staged arrays.  The layer-wise adaptive kinds keep their state rules with their launch sequence
+// (KVStore::EnsureState).
 __host__ __device__ constexpr bool OptHasS0(int kind) {
   return kind == OPT_SGD_MOM || kind == OPT_ADAM || kind == OPT_ADAMW || kind == OPT_ADAM_STD || kind == OPT_NAG ||
-         kind == OPT_ADABELIEF;
+         kind == OPT_ADABELIEF || kind == OPT_RMSPROP || kind == OPT_RMSPROP_CENTERED;
 }
 __host__ __device__ constexpr bool OptHasS1(int kind) {
-  return kind == OPT_ADAM || kind == OPT_ADAMW || kind == OPT_ADAM_STD || kind == OPT_ADABELIEF;
+  return kind == OPT_ADAM || kind == OPT_ADAMW || kind == OPT_ADAM_STD || kind == OPT_ADABELIEF ||
+         kind == OPT_RMSPROP_CENTERED;
 }
+__host__ __device__ constexpr bool OptHasS2(int kind) { return kind == OPT_RMSPROP_CENTERED; }
 
 enum SumOrder : int {
   ORDER_DEVICE = 0,  // ((in0+in1)+in2)+...                  ndarray_function-inl.h:457-486
@@ -89,8 +95,9 @@ struct alignas(16) TensorWork {
     uint32_t tree_prog;  // ORDER_TREE launches (never NVLS): when to add which partial sums, src[] being in the
   };                     //   tree's leaf order (topology.h: ReduceProgram)
   int key;           // host side only: the key this entry belongs to
+  float* s2;         // centered RMSProp momentum (appended: every field above keeps its offset)
 };
-static_assert(sizeof(TensorWork) == 400, "TensorWork layout");
+static_assert(sizeof(TensorWork) == 416, "TensorWork layout");
 
 constexpr int kWorkVec16 = 1;    // every pointer 16-byte aligned and begin % 8 == 0: 16-byte packet loads / stores
 constexpr int kWorkStaged = 2;   // eligible for the shared-memory staged variant (implies kWorkVec16)
@@ -104,7 +111,7 @@ inline int WorkFlags(const TensorWork& t, bool staged) {
   for (int k = 0; k < t.n_src; ++k) low |= reinterpret_cast<uintptr_t>(t.src[k]) & 15;
   for (int k = 0; k < t.n_out; ++k) low |= reinterpret_cast<uintptr_t>(t.out[k]) & 15;
   low |= (reinterpret_cast<uintptr_t>(t.w) | reinterpret_cast<uintptr_t>(t.w32) | reinterpret_cast<uintptr_t>(t.s0) |
-          reinterpret_cast<uintptr_t>(t.s1)) & 15;
+          reinterpret_cast<uintptr_t>(t.s1) | reinterpret_cast<uintptr_t>(t.s2)) & 15;
   if (low != 0) return 0;
   return kWorkVec16 | (staged ? kWorkStaged : 0);
 }
@@ -159,6 +166,8 @@ struct DenseLaunch {
   int nvls_pipe;                 // NVLS variant: 1 = next chunk's ld_reduce issued before this chunk's update/stores
   int mp_arith;                  // 1: a 16-bit key of an optimizer created with multi_precision -- update_one takes
                                  //   the mp_* operator's grouping where it differs from the plain one (Hyper::mp)
+  float rho;                     // RMSProp: decay of the squared-gradient (and centered: gradient) averages
+  float clip_weights;            // RMSProp: |new weight| <= clip_weights when >= 0 (< 0: off)
 };
 
 // returns cudaError_t as int; never throws

@@ -426,7 +426,7 @@ void KVStore::SetOptimizer(const std::string& name, const std::vector<std::pair<
   OptimizerConfig c;
   const std::string n = Lower(name);
   c.enabled = true;
-  bool reset_states = false;
+  bool reset_states = false, centered = false;
   if (n == "sgd") { c.kind = OPT_SGD; c.lr = 0.1; }                             // sgd.py:95
   else if (n == "adam") { c.kind = OPT_ADAM; c.lr = 0.001; }
   else if (n == "adamw") { c.kind = OPT_ADAMW; c.lr = 0.001; c.eps = 1e-6f; }  // adamW.py:80
@@ -436,6 +436,7 @@ void KVStore::SetOptimizer(const std::string& name, const std::vector<std::pair<
   else if (n == "lars") { c.kind = OPT_LARS; c.lr = 0.1; }                     // lars.py:77-79
   else if (n == "nag") { c.kind = OPT_NAG; c.lr = 0.1; c.momentum = 0.9f; }     // nag.py:58
   else if (n == "adabelief") { c.kind = OPT_ADABELIEF; c.lr = 0.001; c.eps = 1e-6f; }   // adabelief.py:79
+  else if (n == "rmsprop") { c.kind = OPT_RMSPROP; c.lr = 0.001; c.momentum = 0.9f; }    // rmsprop.py:70-71
   else MXKV_FATAL() << "optimizer '" << name << "' has no fused kernel; register a Python updater instead";
   for (auto& kv : kwargs) {
     const std::string& k = kv.first;
@@ -460,7 +461,17 @@ void KVStore::SetOptimizer(const std::string& name, const std::vector<std::pair<
     else if (k == "correct_bias") c.correct_bias = (v == "True" || v == "true" || v == "1");
     else if (k == "multi_precision") c.multi_precision = (v == "True" || v == "true" || v == "1");
     else if (k == "reset_states") reset_states = (v == "True" || v == "true" || v == "1");
+    else if (k == "rho") c.rho = std::stof(v);
+    else if (k == "centered") centered = (v == "True" || v == "true" || v == "1");
+    else if (k == "clip_weights") c.clip_weights = (v == "None" || v.empty()) ? -1.f : std::stof(v);
     else MXKV_FATAL() << "unknown optimizer argument '" << k << "'";
+  }
+  if (c.kind == OPT_RMSPROP) {
+    if (centered) c.kind = OPT_RMSPROP_CENTERED;                     // rmspropalex_update, rmsprop.py:175-181
+    // RMSProp.fused_step hands clip_gradient / clip_weights to the operator only when they are truthy
+    // (rmsprop.py:169-172): 0, a negative value or None turns either clip off for this optimizer
+    if (!(c.clip > 0.f)) c.clip = -1.f;
+    if (!(c.clip_weights > 0.f)) c.clip_weights = -1.f;
   }
   if (c.kind == OPT_SGD && c.momentum != 0.f) c.kind = OPT_SGD_MOM;   // sgd.py:213-224
   if (c.kind == OPT_NAG && c.momentum == 0.f) c.kind = OPT_SGD;       // nag.py:59-63,141-154: no state, (mp_)sgd_update
@@ -481,7 +492,7 @@ void KVStore::SetOptimizer(const std::string& name, const std::vector<std::pair<
     for (auto& kv : keys_) {
       KeyState& ks = kv.second;
       for (auto& r : ks.reps) {
-        r.w32 = NDArray(); r.s0 = NDArray(); r.s1 = NDArray();
+        for (auto m : kReplicaState) r.*m = NDArray();
         r.aux0 = NDArray(); r.aux1 = NDArray();
         r.state_fresh = true;
       }
@@ -581,7 +592,10 @@ int KVStore::DefaultDevice() {
   return 0;
 }
 
-static bool HoldsState(const Replica& r) { return !(r.w32.is_none() && r.s0.is_none() && r.s1.is_none()); }
+static bool HoldsState(const Replica& r) {
+  for (auto m : kReplicaState) if (!(r.*m).is_none()) return true;
+  return false;
+}
 
 Replica* KVStore::FindReplica(KeyState& ks, int dev) {
   for (auto& r : ks.reps) if (r.dev == dev) return &r;
@@ -620,9 +634,11 @@ Replica& KVStore::EnsureReplica(KeyState& ks, int dev) {
     Replica& src = holder ? *holder : FreshReplica(ks);
     const Context nctx{kGPU, dev};
     const bool sym = PG() != nullptr;
-    if (!src.w32.is_none()) { nr.w32 = NDArray::Empty(ks.shape, nctx, kFloat32, sym); CopyFromTo(src.w32, nr.w32); }
-    if (!src.s0.is_none()) { nr.s0 = NDArray::Empty(ks.shape, nctx, kFloat32, sym); CopyFromTo(src.s0, nr.s0); }
-    if (!src.s1.is_none()) { nr.s1 = NDArray::Empty(ks.shape, nctx, kFloat32, sym); CopyFromTo(src.s1, nr.s1); }
+    for (auto m : kReplicaState) {
+      if ((src.*m).is_none()) continue;
+      nr.*m = NDArray::Empty(ks.shape, nctx, kFloat32, sym);
+      CopyFromTo(src.*m, nr.*m);
+    }
   } else {
     MXKV_CHECK(!ks.init_value.is_none()) << "key " << ks.key << " has no initial value";
     CopyFromTo(ks.init_value, nr.local);
@@ -640,9 +656,8 @@ void KVStore::SyncState(KeyState& ks, Replica& r) {
   if (r.state_fresh) return;
   for (auto& s : ks.reps) {
     if (&s == &r || !s.state_fresh || !HoldsState(s)) continue;
-    if (!s.w32.is_none() && !r.w32.is_none()) CopyFromTo(s.w32, r.w32);
-    if (!s.s0.is_none() && !r.s0.is_none()) CopyFromTo(s.s0, r.s0);
-    if (!s.s1.is_none() && !r.s1.is_none()) CopyFromTo(s.s1, r.s1);
+    for (auto m : kReplicaState)
+      if (!(s.*m).is_none() && !(r.*m).is_none()) CopyFromTo(s.*m, r.*m);
     r.state_fresh = true;
     return;
   }
@@ -688,6 +703,11 @@ void KVStore::EnsureState(KeyState& ks, Replica& r, bool mp) {
     created = true;
     r.s1 = NDArray::Empty(ks.shape, ctx, kFloat32, sym);
     CUDA_CALL(cudaMemsetAsync(r.s1.data(), 0, r.s1.nbytes(), s));
+  }
+  if (OptHasS2(opt_.kind) && r.s2.is_none()) {
+    created = true;
+    r.s2 = NDArray::Empty(ks.shape, ctx, kFloat32, sym);
+    CUDA_CALL(cudaMemsetAsync(r.s2.data(), 0, r.s2.nbytes(), s));
   }
   // state arrays that come into being after updates have already happened elsewhere start out stale:
   // SyncState fills them from a replica that took part (zeros / a cast of the weight are only right for
@@ -2134,7 +2154,8 @@ void KVStore::LaunchWorks(const LaunchClassKey& ck, std::vector<std::vector<Tens
     int max_src = 1;
     for (int p = my_first; p <= my_last; ++p)
       for (auto& t : per_part[p]) { ok = ok && (t.flags & kWorkStaged); max_src = std::max(max_src, t.n_src); }
-    const int extra = (opt_kind != OPT_NONE ? 1 : 0) + (OptHasS0(opt_kind) ? 1 : 0) + (OptHasS1(opt_kind) ? 1 : 0);
+    const int extra = (opt_kind != OPT_NONE ? 1 : 0) + (OptHasS0(opt_kind) ? 1 : 0) + (OptHasS1(opt_kind) ? 1 : 0) +
+                      (OptHasS2(opt_kind) ? 1 : 0);
     // the staged variant is taken (a) whenever sources are read over NVLink (more bytes in flight
     // against a ~2 us round trip) and (b) locally when a thread of the per-thread variant would have
     // few loads in flight (<= 2 sources, >= 3 streams).  With >= 3 local sources the per-thread variant
@@ -2199,6 +2220,7 @@ void KVStore::LaunchWorks(const LaunchClassKey& ck, std::vector<std::vector<Tens
                     EnvInt("MXKV_B200_FP16_FP32_ACCUM", 0) != 0) ? 1 : 0;
     L.rescale = opt_.rescale; L.clip = opt_.clip; L.momentum = opt_.momentum;
     L.beta1 = static_cast<float>(opt_.beta1); L.beta2 = static_cast<float>(opt_.beta2); L.eps = opt_.eps;
+    L.rho = opt_.rho; L.clip_weights = opt_.clip_weights;
     L.sync.mode = ck.sync_mode;
     L.sync.world = n_part;
     L.sync.rank = p;
@@ -2238,6 +2260,7 @@ TensorWork KVStore::ReplicaWork(const KeyState& ks, const Replica& r, bool mp, i
   tw.w32 = mp ? static_cast<float*>(r.w32.data()) : nullptr;
   tw.s0 = r.s0.is_none() ? nullptr : static_cast<float*>(r.s0.data());
   tw.s1 = r.s1.is_none() ? nullptr : static_cast<float*>(r.s1.data());
+  tw.s2 = r.s2.is_none() ? nullptr : static_cast<float*>(r.s2.data());
   tw.begin = begin; tw.end = end;
   tw.lr = lr; tw.wd = wd; tw.eta = KeyEta(ks); tw.key = ks.key;
   return tw;
@@ -2347,16 +2370,16 @@ void KVStore::RunCallbackUpdater(KeyState& ks, Replica& root, const NDArray& mer
 // python/mxnet/optimizer/updater.py:108-127)
 // ---------------------------------------------------------------------------
 void KVStore::GatherState(KeyState& ks) {
-  // sharded layout -> every replica complete.  Shard p of {w32,s0,s1} is valid on participant p.
+  // sharded layout -> every replica complete.  Shard p of every kReplicaState array is valid on participant p.
   Runtime* rt = Runtime::Get();
   ProcessGroup* pg = PG();
   const int n = ks.state_world;
   if (n <= 1) return;
   const int64_t shard = ShardLen(ks.size, n);
-  auto gather = [&](std::function<NDArray&(Replica&)> sel) {
+  auto gather = [&](ReplicaArray sel) {
     if (pg) {
       Replica& me = ks.reps[0];
-      NDArray& mine = sel(me);
+      NDArray& mine = me.*sel;
       if (mine.is_none()) return;
       rt->WaitAll(); pg->Barrier();
       for (int p = 0; p < n; ++p) {
@@ -2376,8 +2399,8 @@ void KVStore::GatherState(KeyState& ks) {
           Replica* owner = FindReplica(ks, ks.state_devs[p]);      // shard p lives on participant p's GPU
           MXKV_CHECK(owner != nullptr) << "state shard " << p << " of key " << ks.key << " has no replica";
           if (owner == &ks.reps[q]) continue;
-          NDArray& src = sel(*owner);
-          NDArray& dst = sel(ks.reps[q]);
+          NDArray& src = (*owner).*sel;
+          NDArray& dst = ks.reps[q].*sel;
           if (src.is_none() || dst.is_none()) continue;
           const int64_t b = std::min(ks.size, shard * p), e = std::min(ks.size, shard * (p + 1));
           if (e <= b) continue;
@@ -2386,9 +2409,7 @@ void KVStore::GatherState(KeyState& ks) {
       }
     }
   };
-  gather([](Replica& r) -> NDArray& { return r.w32; });
-  gather([](Replica& r) -> NDArray& { return r.s0; });
-  gather([](Replica& r) -> NDArray& { return r.s1; });
+  for (auto m : kReplicaState) gather(m);
   ks.state_world = 0;
   ks.state_devs.clear();
   for (auto& r : ks.reps) r.state_fresh = HoldsState(r);      // every replica with state arrays holds every shard
@@ -2482,12 +2503,8 @@ NDArray KVStore::GetState(bool str_key, int ikey, const std::string& skey, int w
   Replica* holder = nullptr;
   for (auto& cand : ks.reps) if (cand.state_fresh && HoldsState(cand)) { holder = &cand; break; }
   Replica& r = holder ? *holder : FreshReplica(ks);
-  switch (which) {
-    case 1: return r.w32;
-    case 2: return r.s0;
-    case 3: return r.s1;
-  }
-  MXKV_FATAL() << "GetState: which must be 0..3";
+  MXKV_CHECK(which >= 1 && which <= kNumReplicaState) << "GetState: which must be 0.." << kNumReplicaState;
+  return r.*kReplicaState[which - 1];
 }
 
 void KVStore::SetState(bool str_key, int ikey, const std::string& skey, int which, const NDArray& v) {
@@ -2497,17 +2514,11 @@ void KVStore::SetState(bool str_key, int ikey, const std::string& skey, int whic
   if (ks.local_world > 0) GatherLocal(ks);
   GatherState(ks);
   MXKV_CHECK(v.size() == ks.size) << "SetState: size mismatch";
+  MXKV_CHECK(which >= 0 && which <= kNumReplicaState) << "SetState: which must be 0.." << kNumReplicaState;
   for (auto& r : ks.reps) {
-    NDArray* dst = nullptr;
     const bool lowp = ks.dtype == kFloat16 || ks.dtype == kBfloat16;
     if (which != 0) EnsureState(ks, r, opt_.multi_precision || lowp);
-    switch (which) {
-      case 0: dst = &r.local; break;
-      case 1: dst = &r.w32; break;
-      case 2: dst = &r.s0; break;
-      case 3: dst = &r.s1; break;
-      default: MXKV_FATAL() << "SetState: which must be 0..3";
-    }
+    NDArray* dst = which == 0 ? &r.local : &(r.*kReplicaState[which - 1]);
     MXKV_CHECK(!dst->is_none()) << "SetState: the active optimizer has no such state";
     CopyFromTo(v.Reshape(dst->shape()), *dst);
   }

@@ -41,6 +41,7 @@ struct OptimizerConfig {
   bool multi_precision = false;
   bool lazy_update = false;   // row_sparse gradients: touch only the rows present (sgd.py:78, adam.py:77 default False)
   bool correct_bias = true;   // AdamW, AdaBelief (python/mxnet/optimizer/adamW.py:80-88, adabelief.py:79-87)
+  float rho = 0.9f, clip_weights = -1.f;   // RMSProp (rmsprop.py:70-71); clip_weights < 0: off
   // LAMB / LANS / LARS (python/mxnet/optimizer/{lamb,lans,lars}.py)
   float lower_bound = -1.f, upper_bound = -1.f;   // bounds on the weight norm, < 0: not set
   bool bias_correction = true;                     // LAMB
@@ -54,13 +55,13 @@ struct Replica {
   int dev = -1;
   NDArray local;     // the stored value, key dtype
   NDArray w32;       // fp32 master (multi precision)
-  NDArray s0, s1;    // optimizer state
+  NDArray s0, s1, s2;  // optimizer state (kernels.h: OptHasS0 / OptHasS1 / OptHasS2)
   NDArray stage;     // MP mode: symmetric staging for non-symmetric gradients
   NDArray merged;    // updater-callback path: reduce target
   NDArray aux0, aux1;  // LAMB/LANS/LARS: fp32 temporaries between the phases (update direction / merged gradient)
   NDArray nrm;         // LAMB/LANS/LARS: this replica's per-key sums of squares (peer-visible)
   bool fresh = true;
-  bool state_fresh = true;   // optimizer state (w32/s0/s1) reflects every update so far
+  bool state_fresh = true;   // optimizer state (kReplicaState) reflects every update so far
   // row_sparse keys: `local` is the dense-backed table [num_rows x row_len]
   NDArray rsp_merged;            // union ids + summed rows of the last push (capacity n * rsp_cap rows)
   NDArray rsp_first, rsp_pf;     // int32 workspaces of the union kernels
@@ -72,6 +73,12 @@ struct Replica {
   int rsp_n = 0;
   NDArray stage_idx, stage_val, stage_nnz;   // MP mode: symmetric staging of this rank's gradient
 };
+
+// A replica's optimizer-state arrays in the numbering of MXKVB200GetState / SetState (which = 1 + index): the fp32
+// master, state0, state1, state2.  Every copy, gather, reset and presence check of the state walks this one list.
+typedef NDArray Replica::*ReplicaArray;
+inline constexpr ReplicaArray kReplicaState[] = {&Replica::w32, &Replica::s0, &Replica::s1, &Replica::s2};
+constexpr int kNumReplicaState = static_cast<int>(sizeof(kReplicaState) / sizeof(kReplicaState[0]));
 
 struct KeyState {
   int key = 0;
@@ -161,7 +168,8 @@ class KVStore {
                    const std::vector<NDArray>& weights, const std::vector<NDArray>& grads);
   void SetLearningRate(double lr);
   bool has_fused_optimizer() const { return opt_.enabled; }
-  // which: 0 stored value, 1 fp32 master, 2 state0, 3 state1; gathers shards so the result is complete
+  // which: 0 stored value, 1 + i kReplicaState[i] (fp32 master, state0, state1, state2); gathers shards so the
+  // result is complete
   NDArray GetState(bool str_key, int ikey, const std::string& skey, int which);
   void SetState(bool str_key, int ikey, const std::string& skey, int which, const NDArray& v);
   // per-key switches of the fused optimizers; "no_trust_ratio": LARS skips the layer-wise ratio (lars.py:121-123)

@@ -26,6 +26,7 @@ namespace mxkv {
 struct Hyper {
   float lr, wd, eta, rescale, clip, momentum, beta1, beta2, eps;
   bool mp;    // OPT_NAG only: MP_NAGMomKernel's grouping of the weight step (DenseLaunch::mp_arith)
+  float rho, clip_weights;   // OPT_RMSPROP / OPT_RMSPROP_CENTERED (DenseLaunch::rho / clip_weights)
 };
 
 MXKV_HD float clipf(float x, float b) {   // mshadow_op::clip, mshadow_op.h:999-1009
@@ -108,8 +109,40 @@ MXKV_HD float update_one(float g, float w, float& s0, float& s1, const Hyper& h)
     const float v = __fadd_rn(__fadd_rn(__fmul_rn(h.beta2, __fsub_rn(s1, adj)), adj), h.eps);
     s0 = m; s1 = v;
     return __fsub_rn(w, __fmul_rn(h.eta, __fdiv_rn(__fmul_rn(h.lr, m), __fadd_rn(__fsqrt_rn(v), h.eps))));
+  } else if (OPT == OPT_RMSPROP) {
+    // RMSPropUpdateKernel (s0 = var): wd is added AFTER the clip; the weight clip is applied to the new weight
+    float r = __fmul_rn(h.rescale, g);
+    if (h.clip >= 0.0f) r = clipf(r, h.clip);
+    r = __fadd_rn(r, __fmul_rn(h.wd, w));
+    const float n = __fadd_rn(__fmul_rn(__fsub_rn(1.f, h.rho), __fmul_rn(r, r)), __fmul_rn(h.rho, s0));
+    s0 = n;
+    const float wn = __fsub_rn(w, __fdiv_rn(__fmul_rn(h.lr, r), __fadd_rn(__fsqrt_rn(n), h.eps)));
+    return h.clip_weights >= 0.0f ? clipf(wn, h.clip_weights) : wn;
   }
   return g;  // OPT_NONE
+}
+
+// The kinds with a third state array (OptHasS2) are computed here; every other kind is the five-argument form
+// above, and s2 is not touched.
+template <int OPT>
+MXKV_HD float update_one(float g, float w, float& s0, float& s1, float& s2, const Hyper& h) {
+  if constexpr (OPT == OPT_RMSPROP_CENTERED) {
+    // RMSPropAlexUpdateKernel (s0 = mean, s1 = var, s2 = mom):
+    //   n = (1-rho)*r*r + rho*n;  gbar = (1-rho)*r + rho*gbar;  mom = momentum*mom - (lr*r) / sqrt((n - gbar*gbar) + eps)
+    float r = __fmul_rn(h.rescale, g);
+    if (h.clip >= 0.0f) r = clipf(r, h.clip);
+    r = __fadd_rn(r, __fmul_rn(h.wd, w));
+    const float c = __fsub_rn(1.f, h.rho);
+    const float n = __fadd_rn(__fmul_rn(c, __fmul_rn(r, r)), __fmul_rn(h.rho, s1));
+    const float m = __fadd_rn(__fmul_rn(c, r), __fmul_rn(h.rho, s0));
+    const float d = __fsub_rn(__fmul_rn(h.momentum, s2),
+                              __fdiv_rn(__fmul_rn(h.lr, r), __fsqrt_rn(__fadd_rn(__fsub_rn(n, __fmul_rn(m, m)), h.eps))));
+    s0 = m; s1 = n; s2 = d;
+    const float wn = __fadd_rn(w, d);
+    return h.clip_weights >= 0.0f ? clipf(wn, h.clip_weights) : wn;
+  } else {
+    return update_one<OPT>(g, w, s0, s1, h);
+  }
 }
 
 // ---------------------------------------------------------------------------

@@ -65,7 +65,8 @@ __device__ __forceinline__ void tree_packet(const TensorWork& tw, int64_t e, con
   } else {
     constexpr bool HAS_S0 = OptHasS0(OPT);
     constexpr bool HAS_S1 = OptHasS1(OPT);
-    float w[N], s0[N], s1[N];
+    constexpr bool HAS_S2 = OptHasS2(OPT);
+    float w[N], s0[N], s1[N], s2[N];
     if (MP) {
       ldf<N>(tw.w32, e, w);
     } else {
@@ -75,10 +76,12 @@ __device__ __forceinline__ void tree_packet(const TensorWork& tw, int64_t e, con
     }
     if (HAS_S0) ldf<N>(tw.s0, e, s0);
     if (HAS_S1) ldf<N>(tw.s1, e, s1);
+    if (HAS_S2) ldf<N>(tw.s2, e, s2);
 #pragma unroll
-    for (int i = 0; i < N; ++i) wnew[i] = update_one<OPT>(acc[i], w[i], s0[i], s1[i], h);
+    for (int i = 0; i < N; ++i) wnew[i] = update_one<OPT>(acc[i], w[i], s0[i], s1[i], s2[i], h);
     if (HAS_S0) stf<N>(tw.s0, e, s0);
     if (HAS_S1) stf<N>(tw.s1, e, s1);
+    if (HAS_S2) stf<N>(tw.s2, e, s2);
     if (MP) stf<N>(tw.w32, e, wnew);
   }
   const int m = tw.n_out;
@@ -115,7 +118,8 @@ kv_dense_tree_kernel(DenseLaunch L) {
   // 16-byte packets of float32, 8-byte packets (4 elements) of the 16-bit types: with three pending partial sums per
   // element next to a batch of loads, 8 elements per thread would not fit in the 64 registers that keep two blocks
   // of 512 threads resident (the residency the rendezvous grid is sized for)
-  constexpr int NV = sizeof(T) == 2 ? 4 : 16 / sizeof(T);
+  // (float32 keys of centered RMSProp, with three state arrays, take one element at a time for the same reason)
+  constexpr int NV = sizeof(T) == 2 ? 4 : (OptHasS2(OPT) ? 1 : 16 / sizeof(T));
   const bool native_half_add = (sizeof(T) == 2) && !L.fp32_accum && (OPT == OPT_NONE);
   int cur = -1;
   for (int64_t c = blockIdx.x; c < L.total_chunks; c += gridDim.x) {
@@ -124,6 +128,7 @@ kv_dense_tree_kernel(DenseLaunch L) {
     h.lr = tw.lr; h.wd = tw.wd; h.eta = tw.eta;
     h.rescale = L.rescale; h.clip = L.clip; h.momentum = L.momentum;
     h.beta1 = L.beta1; h.beta2 = L.beta2; h.eps = L.eps;
+    h.rho = L.rho; h.clip_weights = L.clip_weights;
     h.mp = sizeof(T) == 2 && L.mp_arith != 0;
 
     const int64_t cb = tw.begin + (c - L.chunk_prefix[lo]) * L.chunk_elems;
@@ -187,6 +192,8 @@ static TreeKernelFn pick_tree_opt(int opt, bool mp, bool allow_non_mp) {
       case OPT_TEST: return kv_dense_tree_kernel<T, OPT_TEST, true>;
       case OPT_NAG: return kv_dense_tree_kernel<T, OPT_NAG, true>;
       case OPT_ADABELIEF: return kv_dense_tree_kernel<T, OPT_ADABELIEF, true>;
+      case OPT_RMSPROP: return kv_dense_tree_kernel<T, OPT_RMSPROP, true>;
+      case OPT_RMSPROP_CENTERED: return kv_dense_tree_kernel<T, OPT_RMSPROP_CENTERED, true>;
       default: return nullptr;
     }
   }
@@ -200,6 +207,8 @@ static TreeKernelFn pick_tree_opt(int opt, bool mp, bool allow_non_mp) {
       case OPT_TEST: return kv_dense_tree_kernel<T, OPT_TEST, false>;
       case OPT_NAG: return kv_dense_tree_kernel<T, OPT_NAG, false>;
       case OPT_ADABELIEF: return kv_dense_tree_kernel<T, OPT_ADABELIEF, false>;
+      case OPT_RMSPROP: return kv_dense_tree_kernel<T, OPT_RMSPROP, false>;
+      case OPT_RMSPROP_CENTERED: return kv_dense_tree_kernel<T, OPT_RMSPROP_CENTERED, false>;
       default: return nullptr;
     }
   }

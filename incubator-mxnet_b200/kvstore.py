@@ -455,7 +455,7 @@ class KVStore(KVStoreBase):
         states = {}
         for k in sorted(self._keys, key=str):
             ent = {}
-            for which, name in ((1, "weight32"), (2, "state0"), (3, "state1")):
+            for which, name in ((1, "weight32"), (2, "state0"), (3, "state1"), (4, "state2")):
                 h = self._state_handle(k, which)
                 if h is not None:
                     ent[name] = h.asnumpy()
@@ -491,7 +491,7 @@ class KVStore(KVStoreBase):
         for k, ent in payload["states"].items():
             if only is not None and k not in only:
                 continue
-            for which, name in ((1, "weight32"), (2, "state0"), (3, "state1")):
+            for which, name in ((1, "weight32"), (2, "state0"), (3, "state1"), (4, "state2")):
                 if name in ent:
                     v = _nd.array(ent[name], dtype=np.float32)
                     if isinstance(k, str):

@@ -1,8 +1,8 @@
-"""Optimizer descriptors mirroring python/mxnet/optimizer/{optimizer,sgd,nag,adam,adamW,adabelief,updater}.py.
+"""Optimizer descriptors mirroring python/mxnet/optimizer/{optimizer,sgd,nag,adam,adamW,adabelief,rmsprop,updater}.py.
 
 Two roles:
 * describe the hyper-parameters of the optimizers that have a fused kernel in the native
-  engine (SGD / SGD-momentum / multi-precision SGD, NAG, Adam, AdamW, AdaBelief, Test, and the layer-wise adaptive
+  engine (SGD / SGD-momentum / multi-precision SGD, NAG, Adam, AdamW, AdaBelief, RMSProp, Test, and the layer-wise adaptive
   LAMB / LANS / LARS) -- ``KVStore.set_optimizer``
   hands them to ``MXKVB200SetOptimizer`` and the update then runs inside the reduce kernel;
 * provide the generic ``Updater`` callback (updater.py:39-93) for any other Optimizer object:
@@ -384,6 +384,63 @@ class AdaBelief(Optimizer):
             w.sub_(lr * (mean / (torch.sqrt(var) + self.epsilon)))
 
 
+@register
+class RMSProp(Optimizer):
+    """python/mxnet/optimizer/rmsprop.py; fused kernels rmsprop_update (Tieleman & Hinton) and, with
+    ``centered=True``, rmspropalex_update (Graves) (src/operator/optimizer_op-inl.h:1905-2031)::
+
+        grad = clip(grad * rescale_grad, clip_gradient) + wd * weight
+        centered=False:  var = rho * var + (1 - rho) * grad**2
+                         weight = weight - lr * grad / (sqrt(var) + epsilon)
+        centered=True:   mean = rho * mean + (1 - rho) * grad;  var = rho * var + (1 - rho) * grad**2
+                         mom = momentum * mom - lr * grad / sqrt(var - mean**2 + epsilon)
+                         weight = weight + mom
+        weight = clip(weight, clip_weights)
+
+    As in ``RMSProp.fused_step`` (rmsprop.py:169-172), the fused update clips only where ``clip_gradient`` /
+    ``clip_weights`` is truthy: 0, a negative value or None turns that clip off."""
+    fused_name = "rmsprop"
+
+    def __init__(self, learning_rate=0.001, rho=0.9, momentum=0.9, epsilon=1e-8, centered=False, clip_weights=None,
+                 **kwargs):
+        super(RMSProp, self).__init__(learning_rate=learning_rate, **kwargs)
+        self.rho, self.momentum, self.epsilon = rho, momentum, epsilon
+        self.centered, self.clip_weights = centered, clip_weights
+
+    def fused_kwargs(self):
+        kw = super(RMSProp, self).fused_kwargs()
+        kw.update(rho=self.rho, momentum=self.momentum, epsilon=self.epsilon, centered=bool(self.centered),
+                  clip_weights=self.clip_weights)
+        return kw
+
+    def create_state(self, index, weight):
+        import torch
+        w = weight.as_torch()
+        if self.centered:        # mean, var, mom
+            return tuple(torch.zeros_like(w, dtype=torch.float32) for _ in range(3))
+        return torch.zeros_like(w, dtype=torch.float32)      # var
+
+    def step(self, indices, weights, grads, states):     # rmsprop.py:90-141
+        import torch
+        for index, weight, grad, state in zip(indices, weights, grads, states):
+            self._update_count(index)
+            lr = self._get_lr(index)
+            w, g = weight.as_torch(), grad.as_torch()
+            g = _prep_grad(self, index, w, g)
+            if not self.centered:
+                var = state
+                var.mul_(self.rho).add_((1 - self.rho) * torch.square(g))
+                w.sub_(lr * (g / (torch.sqrt(var) + self.epsilon)))
+            else:
+                mean, var, mom = state
+                mean.mul_(self.rho).add_((1 - self.rho) * g)
+                var.mul_(self.rho).add_((1 - self.rho) * torch.square(g))
+                mom.mul_(self.momentum).sub_(lr * g / torch.sqrt(var - torch.square(mean) + self.epsilon))
+                w.add_(mom)
+            if self.clip_weights:
+                w.clamp_(-self.clip_weights, self.clip_weights)
+
+
 class _LayerwiseAdaptive(Optimizer):
     """Shared part of LAMB / LANS / LARS: ``skip_nonfinite=True`` asks the store to leave weights and
     state alone when a merged gradient holds inf/nan (the AMP overflow skip, gluon/trainer.py:445-448,
@@ -584,7 +641,7 @@ class NativeUpdater(object):
     """Same call contract as :class:`Updater` (updater.py:39-93; ``index`` / ``grad`` / ``weight`` may be
     lists), but the whole list is updated IN PLACE by one fused launch (sequence) of the native engine
     -- what the reference does with ``multi_sgd_mom_update`` / ``multi_mp_sgd_*`` / ``multi_adamw`` /
-    ``multi_adabelief`` / ``multi_lamb`` / ``multi_lans`` when parameters are not updated on the kvstore (sgd.py:170-213,
+    ``multi_adabelief`` / ``rmsprop_update`` / ``multi_lamb`` / ``multi_lans`` when parameters are not updated on the kvstore (sgd.py:170-213,
     lamb.py:170-215).  One instance serves one device, like ``Trainer._updaters[dev]``."""
 
     def __init__(self, optimizer):

@@ -1,7 +1,9 @@
 """Step time of the fused NAG against fused SGD-momentum at N = 1 (one GPU, one gradient per key), and of NAG through
 the Python `step` (use_fused_step=False, the only way to run NAG before the fused kernel existed).  With
 `--pair adabelief`: the fused AdaBelief against the fused Adam instead (both read g, w, mean, var and write stored w,
-mean, var, out: 32 bytes per float32 element).
+mean, var, out: 32 bytes per float32 element).  With `--pair rmsprop`: the fused RMSProp against the fused SGD-momentum
+(24 bytes per float32 element each), the fused centered RMSProp against the fused Adam (40 against 32 bytes: it reads
+g, w, mean, var, mom and writes stored w, mean, var, mom, out), and RMSProp through the Python `step`.
 
 Two key sets: the bench sweep (9 float32 keys, 2^10 ... 2^26 elements) and ResNet-50's 193 gradient-carrying arrays
 (bench.py: keyset).  Both fused optimizers move the same bytes per element (read g, w, mom; write stored w, mom, out),
@@ -10,7 +12,7 @@ engine's stream (the Python path: host clock around a device synchronise, its to
 dense kernel variant that ran (launch counters), and one step checked against the CPU oracle.  The card's name and
 power limit are read with nvidia-smi in the same call and printed with the numbers.
 
-    python tools/optimizer_rate.py [--pair nag|adabelief] [--steps 200] [--warmup 20] [--rounds 3]
+    python tools/optimizer_rate.py [--pair nag|adabelief|rmsprop] [--steps 200] [--warmup 20] [--rounds 3]
 """
 import argparse
 import ctypes
@@ -31,9 +33,13 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 KW = dict(learning_rate=0.01, momentum=0.9, wd=1e-4)
 KW_ADAPTIVE = dict(learning_rate=0.001, wd=1e-4)
-# --pair: (baseline, optimizer under test); the python step is timed for the NAG pair only
-PAIRS = {"nag": ("sgd", "nag"), "adabelief": ("adam", "adabelief")}
-LABELS = {"sgd": "sgd_momentum", "nag": "nag", "adam": "adam", "adabelief": "adabelief"}
+# --pair: (baseline, optimizer under test) pairs, alternated in one process; the python step is timed for the first
+# optimizer under test where it was the only way to run it (NAG, RMSProp)
+PAIRS = {"nag": [("sgd", "nag")], "adabelief": [("adam", "adabelief")],
+         "rmsprop": [("sgd", "rmsprop"), ("adam", "rmsprop_centered")]}
+PYTHON_STEP = ("nag", "rmsprop")
+LABELS = {"sgd": "sgd_momentum", "nag": "nag", "adam": "adam", "adabelief": "adabelief", "rmsprop": "rmsprop",
+          "rmsprop_centered": "rmsprop (centered)"}
 VARIANTS = ("per_thread", "bulk", "nvls", "tree")
 
 
@@ -61,8 +67,11 @@ class Case(object):
         self.kv = mx.kv.create("device")
         self.kv.init(self.keys, [mx.nd.array(w, mx.gpu(0)) for w in w0])
         self.kw = KW if optname in ("sgd", "nag") else KW_ADAPTIVE
+        if optname.startswith("rmsprop"):
+            self.kw = dict(KW_ADAPTIVE, centered=optname == "rmsprop_centered")
         cls = {"sgd": mx.optimizer.SGD, "nag": mx.optimizer.NAG, "adam": mx.optimizer.Adam,
-               "adabelief": mx.optimizer.AdaBelief}[optname]
+               "adabelief": mx.optimizer.AdaBelief, "rmsprop": mx.optimizer.RMSProp,
+               "rmsprop_centered": mx.optimizer.RMSProp}[optname]
         opt = cls(**dict(self.kw, **({} if fused else {"use_fused_step": False})))
         self.kv.set_optimizer(opt)
         self.grads = [mx.nd.array(g, mx.gpu(0)) for g in self.grads_np]
@@ -85,6 +94,9 @@ class Case(object):
         elif self.optname == "adabelief":
             import adabelief_oracle as A
             oopt = A.OracleAdaBelief(**self.kw)
+        elif self.optname.startswith("rmsprop"):
+            import rmsprop_oracle as R
+            oopt = R.OracleRMSProp(**self.kw)
         else:
             oopt = O.OracleOptimizer(self.optname, **self.kw)
         exact, close = True, True
@@ -138,10 +150,12 @@ def main():
     stream = engine_stream(mx, torch)
     result = {"card": info, "pair": args.pair, "steps": args.steps, "warmup": args.warmup, "rounds": args.rounds,
               "cases": []}
-    base, test = PAIRS[args.pair]
+    pairs = PAIRS[args.pair]
     for ksname in ("sweep", "resnet50"):
         shapes = keyset(ksname)
-        cases = [(base, True), (test, True)] + ([(test, False)] if ksname == "resnet50" and test == "nag" else [])
+        cases = [(o, True) for pair in pairs for o in pair]
+        if ksname == "resnet50" and pairs[0][1] in PYTHON_STEP:
+            cases.append((pairs[0][1], False))
         built = {c: Case(mx, shapes, c[0], c[1]) for c in cases}
         checks = {c: built[c].check() for c in cases}
         times = {c: [] for c in cases}
