@@ -1,6 +1,6 @@
 // device_utils.cuh -- device helpers shared by kernels.cu and norm_kernels.cu: 16-byte global
-// accesses, flag loads/stores of the cross-GPU rendezvous, typed packets, and the per-element
-// arithmetic of the fused optimizers.
+// accesses, flag loads/stores of the cross-GPU rendezvous, typed packets, the per-element
+// arithmetic of the fused optimizers, and the work-entry lookup of the dense kernels.
 #pragma once
 #include "kernels.h"
 #include "optim_math.h"
@@ -270,6 +270,38 @@ template <int N> __device__ __forceinline__ void stf(float* p, int64_t e, const 
       st16(p + e + i, v);
     }
   }
+}
+
+// ---------------------------------------------------------------------------
+// work entries of a dense launch
+// ---------------------------------------------------------------------------
+// chunk -> work entry (uniform across the block); the entry is staged in shared memory when it changes
+__device__ __forceinline__ int find_work(const DenseLaunch& L, int64_t c, int* cur, TensorWork* tw) {
+  int lo = 0, hi = L.nworks - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (L.chunk_prefix[mid] <= c) lo = mid; else hi = mid - 1;
+  }
+  if (lo != *cur) {
+    __syncthreads();
+    const uint4* src = reinterpret_cast<const uint4*>(L.works + lo);
+    uint4* dst = reinterpret_cast<uint4*>(tw);
+    for (int i = threadIdx.x; i < static_cast<int>(sizeof(TensorWork) / 16); i += blockDim.x) dst[i] = src[i];
+    __syncthreads();
+    *cur = lo;
+  }
+  return lo;
+}
+
+// the update's hyper-parameters for one entry: lr / wd / eta are per key, the rest per launch
+__device__ __forceinline__ Hyper make_hyper(const DenseLaunch& L, const TensorWork& tw, bool mp) {
+  Hyper h;
+  h.lr = tw.lr; h.wd = tw.wd; h.eta = tw.eta;
+  h.rescale = L.rescale; h.clip = L.clip; h.momentum = L.momentum;
+  h.beta1 = L.beta1; h.beta2 = L.beta2; h.eps = L.eps;
+  h.rho = L.rho; h.clip_weights = L.clip_weights;
+  h.mp = mp;
+  return h;
 }
 
 }  // namespace mxkv

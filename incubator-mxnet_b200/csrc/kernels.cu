@@ -140,27 +140,8 @@ kv_dense_kernel(DenseLaunch L) {
   const bool native_half_add = (sizeof(T) == 2) && !L.fp32_accum && (OPT == OPT_NONE);
   int cur = -1;
   for (int64_t c = blockIdx.x; c < L.total_chunks; c += gridDim.x) {
-    // chunk -> work entry (uniform across the block)
-    int lo = 0, hi = L.nworks - 1;
-    while (lo < hi) {
-      const int mid = (lo + hi + 1) >> 1;
-      if (L.chunk_prefix[mid] <= c) lo = mid; else hi = mid - 1;
-    }
-    if (lo != cur) {
-      __syncthreads();
-      const uint4* src = reinterpret_cast<const uint4*>(L.works + lo);
-      uint4* dst = reinterpret_cast<uint4*>(&tw);
-      for (int i = threadIdx.x; i < static_cast<int>(sizeof(TensorWork) / 16); i += blockDim.x)
-        dst[i] = src[i];
-      __syncthreads();
-      cur = lo;
-    }
-    Hyper h;
-    h.lr = tw.lr; h.wd = tw.wd; h.eta = tw.eta;
-    h.rescale = L.rescale; h.clip = L.clip; h.momentum = L.momentum;
-    h.beta1 = L.beta1; h.beta2 = L.beta2; h.eps = L.eps;
-    h.rho = L.rho; h.clip_weights = L.clip_weights;
-    h.mp = sizeof(T) == 2 && L.mp_arith != 0;
+    const int lo = find_work(L, c, &cur, &tw);
+    const Hyper h = make_hyper(L, tw, sizeof(T) == 2 && L.mp_arith != 0);
 
     const int64_t cb = tw.begin + (c - L.chunk_prefix[lo]) * L.chunk_elems;
     const int64_t ce = (cb + L.chunk_elems < tw.end) ? cb + L.chunk_elems : tw.end;
@@ -310,7 +291,7 @@ kv_dense_bulk_kernel(DenseLaunch L) {
     const int64_t ce = (cb + tile < w->end) ? cb + tile : w->end;
     const uint32_t bytes = static_cast<uint32_t>(ce - cb) * 4u;
     const int n = w->n_src;
-    const int narr = n + (HAS_W ? 1 : 0) + (HAS_S0 ? 1 : 0) + (HAS_S1 ? 1 : 0) + (HAS_S2 ? 1 : 0);
+    const int narr = n + OptStreams(OPT);
     const int s = static_cast<int>(i % stages);
     unsigned char* base = bulk_smem + static_cast<size_t>(s) * stage_bytes;
     mbar_expect_tx(&full[s], bytes * static_cast<uint32_t>(narr));
@@ -333,25 +314,8 @@ kv_dense_bulk_kernel(DenseLaunch L) {
   int cur = -1;
   for (int64_t i = 0; i < ntiles; ++i) {
     const int64_t c = tile_of(i);
-    int lo = 0, hi = L.nworks - 1;
-    while (lo < hi) {
-      const int mid = (lo + hi + 1) >> 1;
-      if (L.chunk_prefix[mid] <= c) lo = mid; else hi = mid - 1;
-    }
-    if (lo != cur) {
-      __syncthreads();
-      const uint4* src = reinterpret_cast<const uint4*>(L.works + lo);
-      uint4* dst = reinterpret_cast<uint4*>(&tw);
-      for (int t = threadIdx.x; t < static_cast<int>(sizeof(TensorWork) / 16); t += blockDim.x) dst[t] = src[t];
-      __syncthreads();
-      cur = lo;
-    }
-    Hyper h;
-    h.lr = tw.lr; h.wd = tw.wd; h.eta = tw.eta;
-    h.rescale = L.rescale; h.clip = L.clip; h.momentum = L.momentum;
-    h.beta1 = L.beta1; h.beta2 = L.beta2; h.eps = L.eps;
-    h.rho = L.rho; h.clip_weights = L.clip_weights;
-    h.mp = false;                     // float32 keys only
+    const int lo = find_work(L, c, &cur, &tw);
+    const Hyper h = make_hyper(L, tw, false);   // float32 keys only
     const int64_t cb = tw.begin + (c - L.chunk_prefix[lo]) * tile;
     const int64_t ce = (cb + tile < tw.end) ? cb + tile : tw.end;
     const int nvec = static_cast<int>((ce - cb) >> 2);
@@ -423,20 +387,11 @@ kv_dense_bulk_kernel(DenseLaunch L) {
 
 typedef void (*BulkKernelFn)(DenseLaunch);
 static BulkKernelFn pick_bulk(int opt, int mp) {
-  switch (opt) {
-    case OPT_NONE: return kv_dense_bulk_kernel<OPT_NONE, false>;
-    case OPT_SGD: return mp ? kv_dense_bulk_kernel<OPT_SGD, true> : kv_dense_bulk_kernel<OPT_SGD, false>;
-    case OPT_SGD_MOM: return mp ? kv_dense_bulk_kernel<OPT_SGD_MOM, true> : kv_dense_bulk_kernel<OPT_SGD_MOM, false>;
-    case OPT_ADAM: return mp ? kv_dense_bulk_kernel<OPT_ADAM, true> : kv_dense_bulk_kernel<OPT_ADAM, false>;
-    case OPT_ADAMW: return mp ? kv_dense_bulk_kernel<OPT_ADAMW, true> : kv_dense_bulk_kernel<OPT_ADAMW, false>;
-    case OPT_TEST: return mp ? kv_dense_bulk_kernel<OPT_TEST, true> : kv_dense_bulk_kernel<OPT_TEST, false>;
-    case OPT_NAG: return mp ? kv_dense_bulk_kernel<OPT_NAG, true> : kv_dense_bulk_kernel<OPT_NAG, false>;
-    case OPT_ADABELIEF: return mp ? kv_dense_bulk_kernel<OPT_ADABELIEF, true> : kv_dense_bulk_kernel<OPT_ADABELIEF, false>;
-    case OPT_RMSPROP: return mp ? kv_dense_bulk_kernel<OPT_RMSPROP, true> : kv_dense_bulk_kernel<OPT_RMSPROP, false>;
-    case OPT_RMSPROP_CENTERED:
-      return mp ? kv_dense_bulk_kernel<OPT_RMSPROP_CENTERED, true> : kv_dense_bulk_kernel<OPT_RMSPROP_CENTERED, false>;
-    default: return nullptr;
-  }
+  if (opt == OPT_NONE) return kv_dense_bulk_kernel<OPT_NONE, false>;
+  return ElementwiseOpts::Dispatch<BulkKernelFn>(opt, [&](auto k) {
+    constexpr int K = decltype(k)::value;
+    return mp ? kv_dense_bulk_kernel<K, true> : kv_dense_bulk_kernel<K, false>;
+  });
 }
 
 // ---------------------------------------------------------------------------
@@ -541,12 +496,7 @@ kv_dense_nvls_kernel(DenseLaunch L) {
       __syncthreads();
       cur = k.lo;
     }
-    Hyper h;
-    h.lr = tw.lr; h.wd = tw.wd; h.eta = tw.eta;
-    h.rescale = L.rescale; h.clip = L.clip; h.momentum = L.momentum;
-    h.beta1 = L.beta1; h.beta2 = L.beta2; h.eps = L.eps;
-    h.rho = L.rho; h.clip_weights = L.clip_weights;
-    h.mp = false;                     // float32 keys only
+    const Hyper h = make_hyper(L, tw, false);   // float32 keys only
     const int64_t nvec = (k.ce - k.cb) >> 2;
     const int n_plain = tw.n_out - tw.n_mc;
     // state of all U packets first (independent HBM loads in flight together), then the arithmetic
@@ -599,23 +549,11 @@ typedef void (*NvlsKernelFn)(DenseLaunch);
 
 template <int U, bool PIPE>
 static NvlsKernelFn pick_nvls_opt(int opt, int mp) {
-  switch (opt) {
-    case OPT_NONE: return kv_dense_nvls_kernel<OPT_NONE, false, U, PIPE>;
-    case OPT_SGD: return mp ? kv_dense_nvls_kernel<OPT_SGD, true, U, PIPE> : kv_dense_nvls_kernel<OPT_SGD, false, U, PIPE>;
-    case OPT_SGD_MOM: return mp ? kv_dense_nvls_kernel<OPT_SGD_MOM, true, U, PIPE> : kv_dense_nvls_kernel<OPT_SGD_MOM, false, U, PIPE>;
-    case OPT_ADAM: return mp ? kv_dense_nvls_kernel<OPT_ADAM, true, U, PIPE> : kv_dense_nvls_kernel<OPT_ADAM, false, U, PIPE>;
-    case OPT_ADAMW: return mp ? kv_dense_nvls_kernel<OPT_ADAMW, true, U, PIPE> : kv_dense_nvls_kernel<OPT_ADAMW, false, U, PIPE>;
-    case OPT_TEST: return mp ? kv_dense_nvls_kernel<OPT_TEST, true, U, PIPE> : kv_dense_nvls_kernel<OPT_TEST, false, U, PIPE>;
-    case OPT_NAG: return mp ? kv_dense_nvls_kernel<OPT_NAG, true, U, PIPE> : kv_dense_nvls_kernel<OPT_NAG, false, U, PIPE>;
-    case OPT_ADABELIEF:
-      return mp ? kv_dense_nvls_kernel<OPT_ADABELIEF, true, U, PIPE> : kv_dense_nvls_kernel<OPT_ADABELIEF, false, U, PIPE>;
-    case OPT_RMSPROP:
-      return mp ? kv_dense_nvls_kernel<OPT_RMSPROP, true, U, PIPE> : kv_dense_nvls_kernel<OPT_RMSPROP, false, U, PIPE>;
-    case OPT_RMSPROP_CENTERED:
-      return mp ? kv_dense_nvls_kernel<OPT_RMSPROP_CENTERED, true, U, PIPE>
-                : kv_dense_nvls_kernel<OPT_RMSPROP_CENTERED, false, U, PIPE>;
-    default: return nullptr;
-  }
+  if (opt == OPT_NONE) return kv_dense_nvls_kernel<OPT_NONE, false, U, PIPE>;
+  return ElementwiseOpts::Dispatch<NvlsKernelFn>(opt, [&](auto k) {
+    constexpr int K = decltype(k)::value;
+    return mp ? kv_dense_nvls_kernel<K, true, U, PIPE> : kv_dense_nvls_kernel<K, false, U, PIPE>;
+  });
 }
 
 // Centered RMSProp (four state packets per gradient packet) at the default point U = 2 spills 120 / 96 bytes
@@ -703,57 +641,33 @@ typedef void (*DenseKernelFn)(DenseLaunch);
 
 template <typename T, int OPT, bool MP>
 static DenseKernelFn pick_n(bool small_n) {
-  // the two-packet variant is only instantiated where it stays inside 64 registers
-  if constexpr (OPT == OPT_NONE || OPT == OPT_SGD || OPT == OPT_TEST) {
+  if constexpr (OptHasSmallN(OPT)) {
     if (small_n) return kv_dense_kernel<T, OPT, MP, true>;
   }
   return kv_dense_kernel<T, OPT, MP, false>;
 }
 
 template <typename T>
-static DenseKernelFn pick_opt(int opt, bool mp, bool small_n, bool allow_non_mp) {
+static DenseKernelFn pick_opt(int opt, bool mp, bool small_n) {
   if (opt == OPT_NONE) return pick_n<T, OPT_NONE, false>(small_n);
-  if (mp) {
-    switch (opt) {
-      case OPT_SGD: return pick_n<T, OPT_SGD, true>(small_n);
-      case OPT_SGD_MOM: return pick_n<T, OPT_SGD_MOM, true>(small_n);
-      case OPT_ADAM: return pick_n<T, OPT_ADAM, true>(small_n);
-      case OPT_ADAMW: return pick_n<T, OPT_ADAMW, true>(small_n);
-      case OPT_TEST: return pick_n<T, OPT_TEST, true>(small_n);
-      case OPT_NAG: return pick_n<T, OPT_NAG, true>(small_n);
-      case OPT_ADABELIEF: return pick_n<T, OPT_ADABELIEF, true>(small_n);
-      case OPT_RMSPROP: return pick_n<T, OPT_RMSPROP, true>(small_n);
-      case OPT_RMSPROP_CENTERED: return pick_n<T, OPT_RMSPROP_CENTERED, true>(small_n);
-      default: return nullptr;
-    }
-  }
-  if (!allow_non_mp) return nullptr;
-  return nullptr;
+  return ElementwiseOpts::Dispatch<DenseKernelFn>(opt, [&](auto k) -> DenseKernelFn {
+    constexpr int K = decltype(k)::value;
+    if (mp) return pick_n<T, K, true>(small_n);
+    if constexpr (sizeof(T) == 4) return pick_n<T, K, false>(small_n);   // 16-bit keys: fp32 master only
+    return nullptr;
+  });
 }
 
 static DenseKernelFn pick_kernel(const DenseLaunch& L) {
   const bool mp = L.multi_precision != 0;
-  // the two-packet variant stays inside 64 registers (2 resident blocks/SM) only for these
-  const bool sn = L.small_n != 0 && (L.opt == OPT_NONE || L.opt == OPT_SGD || L.opt == OPT_TEST);
+  const bool sn = L.small_n != 0 && OptHasSmallN(L.opt);
   switch (L.dtype) {
     case kFloat32:
-      if (mp || L.opt == OPT_NONE) return pick_opt<float>(L.opt, mp, sn, true);
-      switch (L.opt) {
-        case OPT_SGD: return pick_n<float, OPT_SGD, false>(sn);
-        case OPT_SGD_MOM: return pick_n<float, OPT_SGD_MOM, false>(sn);
-        case OPT_ADAM: return pick_n<float, OPT_ADAM, false>(sn);
-        case OPT_ADAMW: return pick_n<float, OPT_ADAMW, false>(sn);
-        case OPT_TEST: return pick_n<float, OPT_TEST, false>(sn);
-        case OPT_NAG: return pick_n<float, OPT_NAG, false>(sn);
-        case OPT_ADABELIEF: return pick_n<float, OPT_ADABELIEF, false>(sn);
-        case OPT_RMSPROP: return pick_n<float, OPT_RMSPROP, false>(sn);
-        case OPT_RMSPROP_CENTERED: return pick_n<float, OPT_RMSPROP_CENTERED, false>(sn);
-        case OPT_SGD_STD: return kv_dense_kernel<float, OPT_SGD_STD, false, false>;
-        case OPT_ADAM_STD: return kv_dense_kernel<float, OPT_ADAM_STD, false, false>;
-        default: return nullptr;
-      }
-    case kFloat16: return pick_opt<__half>(L.opt, mp, sn, false);
-    case kBfloat16: return pick_opt<__nv_bfloat16>(L.opt, mp, sn, false);
+      if (!mp && L.opt == OPT_SGD_STD) return kv_dense_kernel<float, OPT_SGD_STD, false, false>;
+      if (!mp && L.opt == OPT_ADAM_STD) return kv_dense_kernel<float, OPT_ADAM_STD, false, false>;
+      return pick_opt<float>(L.opt, mp, sn);
+    case kFloat16: return pick_opt<__half>(L.opt, mp, sn);
+    case kBfloat16: return pick_opt<__nv_bfloat16>(L.opt, mp, sn);
     case kFloat64: return L.opt == OPT_NONE ? kv_sum_typed_kernel<double> : nullptr;
     case kInt32: return L.opt == OPT_NONE ? kv_sum_typed_kernel<int32_t> : nullptr;
     case kInt64: return L.opt == OPT_NONE ? kv_sum_typed_kernel<int64_t> : nullptr;

@@ -9,6 +9,7 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <type_traits>
 
 namespace mxkv {
 
@@ -61,6 +62,32 @@ __host__ __device__ constexpr bool OptHasS1(int kind) {
          kind == OPT_RMSPROP_CENTERED;
 }
 __host__ __device__ constexpr bool OptHasS2(int kind) { return kind == OPT_RMSPROP_CENTERED; }
+// The fp32 arrays a kind streams next to its gradients: the weight (every kind but OPT_NONE) and its state arrays.
+// The staged kernel stages exactly these per tile.
+__host__ __device__ constexpr int OptStreams(int kind) {
+  return (kind != OPT_NONE ? 1 : 0) + (OptHasS0(kind) ? 1 : 0) + (OptHasS1(kind) ? 1 : 0) + (OptHasS2(kind) ? 1 : 0);
+}
+// The kinds whose per-thread kernel also has the two-packets-in-flight variant (DenseLaunch::small_n): only these
+// stay inside the 64 registers that keep two blocks of 512 threads resident with it.
+__host__ __device__ constexpr bool OptHasSmallN(int kind) {
+  return kind == OPT_NONE || kind == OPT_SGD || kind == OPT_TEST;
+}
+
+// The element-wise kinds: every dense kernel (per-thread, staged, multicast, tree) is instantiated for each of them,
+// with and without an fp32 master weight.  OPT_NONE and the float32 per-thread-only *_STD kinds are selected apart.
+// Dispatch<R>(opt, f) returns f(std::integral_constant<int, opt>{}) when opt is in the list, R{} otherwise: the one
+// runtime-to-template step of every kernel selection.
+template <int... K>
+struct OptKinds {
+  template <typename R, typename F>
+  static R Dispatch(int opt, F f) {
+    R r{};
+    (void)((opt == K && (r = f(std::integral_constant<int, K>{}), true)) || ...);
+    return r;
+  }
+};
+using ElementwiseOpts = OptKinds<OPT_SGD, OPT_SGD_MOM, OPT_ADAM, OPT_ADAMW, OPT_TEST, OPT_NAG, OPT_ADABELIEF,
+                                 OPT_RMSPROP, OPT_RMSPROP_CENTERED>;
 
 enum SumOrder : int {
   ORDER_DEVICE = 0,  // ((in0+in1)+in2)+...                  ndarray_function-inl.h:457-486

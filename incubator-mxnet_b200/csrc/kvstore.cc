@@ -2154,8 +2154,7 @@ void KVStore::LaunchWorks(const LaunchClassKey& ck, std::vector<std::vector<Tens
     int max_src = 1;
     for (int p = my_first; p <= my_last; ++p)
       for (auto& t : per_part[p]) { ok = ok && (t.flags & kWorkStaged); max_src = std::max(max_src, t.n_src); }
-    const int extra = (opt_kind != OPT_NONE ? 1 : 0) + (OptHasS0(opt_kind) ? 1 : 0) + (OptHasS1(opt_kind) ? 1 : 0) +
-                      (OptHasS2(opt_kind) ? 1 : 0);
+    const int extra = OptStreams(opt_kind);
     // the staged variant is taken (a) whenever sources are read over NVLink (more bytes in flight
     // against a ~2 us round trip) and (b) locally when a thread of the per-thread variant would have
     // few loads in flight (<= 2 sources, >= 3 streams).  With >= 3 local sources the per-thread variant

@@ -88,24 +88,6 @@ __device__ __forceinline__ void tree_packet(const TensorWork& tw, int64_t e, con
   for (int j = 0; j < m; ++j) P::store(tw.out[j], e, wnew);
 }
 
-// chunk -> work entry (uniform across the block); the entry is staged in shared memory when it changes
-__device__ __forceinline__ int find_work(const DenseLaunch& L, int64_t c, int* cur, TensorWork* tw) {
-  int lo = 0, hi = L.nworks - 1;
-  while (lo < hi) {
-    const int mid = (lo + hi + 1) >> 1;
-    if (L.chunk_prefix[mid] <= c) lo = mid; else hi = mid - 1;
-  }
-  if (lo != *cur) {
-    __syncthreads();
-    const uint4* src = reinterpret_cast<const uint4*>(L.works + lo);
-    uint4* dst = reinterpret_cast<uint4*>(tw);
-    for (int i = threadIdx.x; i < static_cast<int>(sizeof(TensorWork) / 16); i += blockDim.x) dst[i] = src[i];
-    __syncthreads();
-    *cur = lo;
-  }
-  return lo;
-}
-
 }  // namespace
 
 template <typename T, int OPT, bool MP>
@@ -124,12 +106,7 @@ kv_dense_tree_kernel(DenseLaunch L) {
   int cur = -1;
   for (int64_t c = blockIdx.x; c < L.total_chunks; c += gridDim.x) {
     const int lo = find_work(L, c, &cur, &tw);
-    Hyper h;
-    h.lr = tw.lr; h.wd = tw.wd; h.eta = tw.eta;
-    h.rescale = L.rescale; h.clip = L.clip; h.momentum = L.momentum;
-    h.beta1 = L.beta1; h.beta2 = L.beta2; h.eps = L.eps;
-    h.rho = L.rho; h.clip_weights = L.clip_weights;
-    h.mp = sizeof(T) == 2 && L.mp_arith != 0;
+    const Hyper h = make_hyper(L, tw, sizeof(T) == 2 && L.mp_arith != 0);
 
     const int64_t cb = tw.begin + (c - L.chunk_prefix[lo]) * L.chunk_elems;
     const int64_t ce = (cb + L.chunk_elems < tw.end) ? cb + L.chunk_elems : tw.end;
@@ -181,38 +158,14 @@ kv_sum_tree_f64_kernel(DenseLaunch L) {
 typedef void (*TreeKernelFn)(DenseLaunch);
 
 template <typename T>
-static TreeKernelFn pick_tree_opt(int opt, bool mp, bool allow_non_mp) {
+static TreeKernelFn pick_tree_opt(int opt, bool mp) {
   if (opt == OPT_NONE) return kv_dense_tree_kernel<T, OPT_NONE, false>;
-  if (mp) {
-    switch (opt) {
-      case OPT_SGD: return kv_dense_tree_kernel<T, OPT_SGD, true>;
-      case OPT_SGD_MOM: return kv_dense_tree_kernel<T, OPT_SGD_MOM, true>;
-      case OPT_ADAM: return kv_dense_tree_kernel<T, OPT_ADAM, true>;
-      case OPT_ADAMW: return kv_dense_tree_kernel<T, OPT_ADAMW, true>;
-      case OPT_TEST: return kv_dense_tree_kernel<T, OPT_TEST, true>;
-      case OPT_NAG: return kv_dense_tree_kernel<T, OPT_NAG, true>;
-      case OPT_ADABELIEF: return kv_dense_tree_kernel<T, OPT_ADABELIEF, true>;
-      case OPT_RMSPROP: return kv_dense_tree_kernel<T, OPT_RMSPROP, true>;
-      case OPT_RMSPROP_CENTERED: return kv_dense_tree_kernel<T, OPT_RMSPROP_CENTERED, true>;
-      default: return nullptr;
-    }
-  }
-  if (!allow_non_mp) return nullptr;
-  if constexpr (sizeof(T) == 4) {
-    switch (opt) {
-      case OPT_SGD: return kv_dense_tree_kernel<T, OPT_SGD, false>;
-      case OPT_SGD_MOM: return kv_dense_tree_kernel<T, OPT_SGD_MOM, false>;
-      case OPT_ADAM: return kv_dense_tree_kernel<T, OPT_ADAM, false>;
-      case OPT_ADAMW: return kv_dense_tree_kernel<T, OPT_ADAMW, false>;
-      case OPT_TEST: return kv_dense_tree_kernel<T, OPT_TEST, false>;
-      case OPT_NAG: return kv_dense_tree_kernel<T, OPT_NAG, false>;
-      case OPT_ADABELIEF: return kv_dense_tree_kernel<T, OPT_ADABELIEF, false>;
-      case OPT_RMSPROP: return kv_dense_tree_kernel<T, OPT_RMSPROP, false>;
-      case OPT_RMSPROP_CENTERED: return kv_dense_tree_kernel<T, OPT_RMSPROP_CENTERED, false>;
-      default: return nullptr;
-    }
-  }
-  return nullptr;
+  return ElementwiseOpts::Dispatch<TreeKernelFn>(opt, [&](auto k) -> TreeKernelFn {
+    constexpr int K = decltype(k)::value;
+    if (mp) return kv_dense_tree_kernel<T, K, true>;
+    if constexpr (sizeof(T) == 4) return kv_dense_tree_kernel<T, K, false>;   // 16-bit keys: fp32 master only
+    return nullptr;
+  });
 }
 
 // 1 when a tree kernel exists for this dtype / optimizer / precision mode (the host decides per key whether the
@@ -220,9 +173,9 @@ static TreeKernelFn pick_tree_opt(int opt, bool mp, bool allow_non_mp) {
 int TreeKernelAvailable(int dtype, int opt, int multi_precision) {
   const bool mp = multi_precision != 0;
   switch (dtype) {
-    case kFloat32: return pick_tree_opt<float>(opt, mp, true) != nullptr;
-    case kFloat16: return pick_tree_opt<__half>(opt, mp, false) != nullptr;
-    case kBfloat16: return pick_tree_opt<__nv_bfloat16>(opt, mp, false) != nullptr;
+    case kFloat32: return pick_tree_opt<float>(opt, mp) != nullptr;
+    case kFloat16: return pick_tree_opt<__half>(opt, mp) != nullptr;
+    case kBfloat16: return pick_tree_opt<__nv_bfloat16>(opt, mp) != nullptr;
     case kFloat64: return opt == OPT_NONE;
     default: return 0;
   }
@@ -232,9 +185,9 @@ int LaunchDenseTree(const DenseLaunch& L, cudaStream_t stream) {
   const bool mp = L.multi_precision != 0;
   TreeKernelFn fn = nullptr;
   switch (L.dtype) {
-    case kFloat32: fn = pick_tree_opt<float>(L.opt, mp, true); break;
-    case kFloat16: fn = pick_tree_opt<__half>(L.opt, mp, false); break;
-    case kBfloat16: fn = pick_tree_opt<__nv_bfloat16>(L.opt, mp, false); break;
+    case kFloat32: fn = pick_tree_opt<float>(L.opt, mp); break;
+    case kFloat16: fn = pick_tree_opt<__half>(L.opt, mp); break;
+    case kBfloat16: fn = pick_tree_opt<__nv_bfloat16>(L.opt, mp); break;
     case kFloat64: fn = L.opt == OPT_NONE ? kv_sum_tree_f64_kernel : nullptr; break;
     default: break;
   }
