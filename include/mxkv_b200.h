@@ -143,14 +143,17 @@ MXKV_DLL int MXKVStoreSendCommmandToServers(KVStoreHandle handle, int cmd_id, co
 /* ---- MXKVB200 extensions -------------------------------------------------- */
 /* Fused optimizer: what Python's Updater + sgd_update/adam_update ops do per key in the
  * reference (python/mxnet/optimizer/updater.py:39-93) happens inside the reduce kernel.
- * name: "sgd" | "nag" | "adam" | "adamw" | "adabelief" | "rmsprop" | "test" | "lamb" | "lans" | "lars"; kwargs use
- * the reference's hyper-parameter names (learning_rate, wd, momentum, rescale_grad, clip_gradient, beta1, beta2,
- * epsilon, eta, multi_precision, lazy_update, correct_bias, lower_bound, upper_bound,
- * bias_correction, rho, centered, clip_weights).  rmsprop: centered=True selects rmspropalex_update; a
+ * name: "sgd" | "nag" | "adam" | "adamw" | "adabelief" | "rmsprop" | "signum" | "test" | "lamb" | "lans" | "lars";
+ * kwargs use the reference's hyper-parameter names (learning_rate, wd, momentum, rescale_grad, clip_gradient, beta1,
+ * beta2, epsilon, eta, multi_precision, lazy_update, correct_bias, lower_bound, upper_bound,
+ * bias_correction, rho, centered, clip_weights, wd_lh).  rmsprop: centered=True selects rmspropalex_update; a
  * clip_gradient or clip_weights of 0, below 0 or None turns that clip off, as RMSProp.fused_step passes them only
- * when they are truthy.  lamb / lans / lars additionally take skip_nonfinite=True: when any merged
- * gradient of a push holds inf/nan, that push changes neither weights nor optimizer state (the AMP
- * overflow skip of gluon/trainer.py:445-448, decided on the device inside the same launch sequence). */
+ * when they are truthy.  signum: momentum 0 selects signsgd_update (no state; the sign of the summed gradient, wd
+ * + wd_lh as its weight decay, rescale_grad and clip_gradient unused), any other momentum signum_update (a negative
+ * one runs it at momentum 0); clip_gradient is off at 0, below 0 or None, as for rmsprop.  lamb / lans / lars
+ * additionally take skip_nonfinite=True: when any merged gradient of a push holds inf/nan, that push changes neither
+ * weights nor optimizer state (the AMP overflow skip of gluon/trainer.py:445-448, decided on the device inside the
+ * same launch sequence). */
 MXKV_DLL int MXKVB200SetOptimizer(KVStoreHandle handle, const char* name, uint32_t num_params,
                                   const char** keys, const char** vals);
 MXKV_DLL int MXKVB200SetLearningRate(KVStoreHandle handle, double lr);
@@ -161,7 +164,8 @@ MXKV_DLL int MXKVB200SetOptimizerMult(KVStoreHandle handle, int key, const char*
  * 39-93) and of the multi-tensor update operators it ends in when parameters are NOT updated on the
  * kvstore (multi_sgd_update / multi_sgd_mom_update / multi_mp_sgd_*, src/operator/optimizer_op-inl.h:
  * 207-375; nag_mom_update / mp_nag_mom_update per weight, :1029-1092; multi_adamw, multi_adabelief,
- * multi_lamb, multi_lans; rmsprop_update / rmspropalex_update per weight, :1905-2031).  Create the handle with MXKVStoreCreate("updater"), give it an optimizer with MXKVB200SetOptimizer, then every call updates all (weight, grad) pairs
+ * multi_lamb, multi_lans; rmsprop_update / rmspropalex_update per weight, :1905-2031; signsgd_update /
+ * signum_update per weight, :2293-2379).  Create the handle with MXKVStoreCreate("updater"), give it an optimizer with MXKVB200SetOptimizer, then every call updates all (weight, grad) pairs
  * IN PLACE with one launch (sequence) on their GPU.  Optimizer state of an index is created on first
  * sight and is reachable through MXKVB200GetState / SetState / Get|SetUpdateCount.  One handle serves
  * one device, like the reference's `Trainer._updaters[dev]`.  Never collective.  grads == NULL only
@@ -189,7 +193,8 @@ MXKV_DLL int MXKVB200GetOverflow(KVStoreHandle handle, int* out);
  * out[0] = 0 if any element of any array is inf/nan (init_output != 0: out[0] is set to 1 first). */
 MXKV_DLL int MXKVB200MultiSumSq(uint32_t num, NDArrayHandle* arrays, float scale, NDArrayHandle out);
 MXKV_DLL int MXKVB200MultiAllFinite(uint32_t num, NDArrayHandle* arrays, int init_output, NDArrayHandle out);
-/* which: 0 stored value, 1 fp32 master weight, 2 state0 (momentum | mean | RMSProp var; centered RMSProp: mean),
+/* which: 0 stored value, 1 fp32 master weight, 2 state0 (momentum | mean | RMSProp var; centered RMSProp: mean;
+ * Signum: the negated momentum, as the reference stores it),
  * 3 state1 (variance), 4 state2 (centered RMSProp momentum).
  * Returns a NEW handle aliasing engine memory (free it with MXNDArrayFree); *out = NULL when the
  * state does not exist. */

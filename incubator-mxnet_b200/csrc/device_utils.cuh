@@ -300,6 +300,7 @@ __device__ __forceinline__ Hyper make_hyper(const DenseLaunch& L, const TensorWo
   h.rescale = L.rescale; h.clip = L.clip; h.momentum = L.momentum;
   h.beta1 = L.beta1; h.beta2 = L.beta2; h.eps = L.eps;
   h.rho = L.rho; h.clip_weights = L.clip_weights;
+  h.wd_lh = L.wd_lh;
   h.mp = mp;
   return h;
 }

@@ -701,8 +701,8 @@ int DenseMaxGrid(int device, int threads) {
 // Function attributes are per device: opt in to large dynamic shared memory on the GPU a launch goes to -- and
 // only there (a process that owns one GPU must not create contexts on the others).  The device must be current.
 static bool EnsureBulkAttr(int device, int opt, int multi_precision) {
-  static bool attr_done[64][32] = {{false}};
-  if (device < 0 || device >= 64 || opt < 0 || opt >= 16) return false;
+  static bool attr_done[64][2 * kNumOptKinds] = {{false}};
+  if (device < 0 || device >= 64 || opt < 0 || opt >= kNumOptKinds) return false;
   const int slot = opt * 2 + (multi_precision ? 1 : 0);
   if (attr_done[device][slot]) return true;
   BulkKernelFn fn = pick_bulk(opt, multi_precision);

@@ -44,18 +44,21 @@ enum OptKind : int {
   OPT_NAG = 11,     // NAGMomKernel / MP_NAGMomKernel        optimizer_op-inl.h:1029-1044,1066-1090
   OPT_ADABELIEF = 12, // MultiMPAdaBeliefKernel              contrib/adabelief-inl.h:354-384
   OPT_RMSPROP = 13,   // RMSPropUpdateKernel                 optimizer_op-inl.h:2005-2031
-  OPT_RMSPROP_CENTERED = 14  // RMSPropAlexUpdateKernel      optimizer_op-inl.h:1905-1939
+  OPT_RMSPROP_CENTERED = 14, // RMSPropAlexUpdateKernel      optimizer_op-inl.h:1905-1939
+  OPT_SIGNSGD = 15,   // SignSGDKernel                       optimizer_op-inl.h:2293-2305
+  OPT_SIGNUM = 16     // SignumKernel                        optimizer_op-inl.h:2361-2379
 };
+constexpr int kNumOptKinds = OPT_SIGNUM + 1;   // one past the last kind: the size of tables indexed by kind
 inline bool IsNormOpt(int kind) { return kind == OPT_LAMB || kind == OPT_LANS || kind == OPT_LARS; }
 
 // The fp32 state arrays an element-wise kind streams through update_one: s0 (momentum / mean / RMSProp var;
-// centered RMSProp: mean), s1 (variance), s2 (centered RMSProp: momentum) -- the tuple order of the reference's
-// create_state.  Every dense kernel loads and stores exactly these, and the staged kernel counts them among its
-// staged arrays.  The layer-wise adaptive kinds keep their state rules with their launch sequence
-// (KVStore::EnsureState).
+// centered RMSProp: mean; Signum: the negated momentum), s1 (variance), s2 (centered RMSProp: momentum) -- the
+// tuple order of the reference's create_state.  Every dense kernel loads and stores exactly these, and the staged
+// kernel counts them among its staged arrays.  The layer-wise adaptive kinds keep their state rules with their launch
+// sequence (KVStore::EnsureState).
 __host__ __device__ constexpr bool OptHasS0(int kind) {
   return kind == OPT_SGD_MOM || kind == OPT_ADAM || kind == OPT_ADAMW || kind == OPT_ADAM_STD || kind == OPT_NAG ||
-         kind == OPT_ADABELIEF || kind == OPT_RMSPROP || kind == OPT_RMSPROP_CENTERED;
+         kind == OPT_ADABELIEF || kind == OPT_RMSPROP || kind == OPT_RMSPROP_CENTERED || kind == OPT_SIGNUM;
 }
 __host__ __device__ constexpr bool OptHasS1(int kind) {
   return kind == OPT_ADAM || kind == OPT_ADAMW || kind == OPT_ADAM_STD || kind == OPT_ADABELIEF ||
@@ -87,7 +90,7 @@ struct OptKinds {
   }
 };
 using ElementwiseOpts = OptKinds<OPT_SGD, OPT_SGD_MOM, OPT_ADAM, OPT_ADAMW, OPT_TEST, OPT_NAG, OPT_ADABELIEF,
-                                 OPT_RMSPROP, OPT_RMSPROP_CENTERED>;
+                                 OPT_RMSPROP, OPT_RMSPROP_CENTERED, OPT_SIGNSGD, OPT_SIGNUM>;
 
 enum SumOrder : int {
   ORDER_DEVICE = 0,  // ((in0+in1)+in2)+...                  ndarray_function-inl.h:457-486
@@ -195,6 +198,7 @@ struct DenseLaunch {
                                  //   the mp_* operator's grouping where it differs from the plain one (Hyper::mp)
   float rho;                     // RMSProp: decay of the squared-gradient (and centered: gradient) averages
   float clip_weights;            // RMSProp: |new weight| <= clip_weights when >= 0 (< 0: off)
+  float wd_lh;                   // Signum: decoupled weight decay, w *= 1 - lr*wd_lh before the sign step
 };
 
 // returns cudaError_t as int; never throws

@@ -437,6 +437,7 @@ void KVStore::SetOptimizer(const std::string& name, const std::vector<std::pair<
   else if (n == "nag") { c.kind = OPT_NAG; c.lr = 0.1; c.momentum = 0.9f; }     // nag.py:58
   else if (n == "adabelief") { c.kind = OPT_ADABELIEF; c.lr = 0.001; c.eps = 1e-6f; }   // adabelief.py:79
   else if (n == "rmsprop") { c.kind = OPT_RMSPROP; c.lr = 0.001; c.momentum = 0.9f; }    // rmsprop.py:70-71
+  else if (n == "signum") { c.kind = OPT_SIGNUM; c.lr = 0.01; c.momentum = 0.9f; }      // signum.py:67
   else MXKV_FATAL() << "optimizer '" << name << "' has no fused kernel; register a Python updater instead";
   for (auto& kv : kwargs) {
     const std::string& k = kv.first;
@@ -464,6 +465,7 @@ void KVStore::SetOptimizer(const std::string& name, const std::vector<std::pair<
     else if (k == "rho") c.rho = std::stof(v);
     else if (k == "centered") centered = (v == "True" || v == "true" || v == "1");
     else if (k == "clip_weights") c.clip_weights = (v == "None" || v.empty()) ? -1.f : std::stof(v);
+    else if (k == "wd_lh") c.wd_lh = std::stod(v);
     else MXKV_FATAL() << "unknown optimizer argument '" << k << "'";
   }
   if (c.kind == OPT_RMSPROP) {
@@ -472,6 +474,14 @@ void KVStore::SetOptimizer(const std::string& name, const std::vector<std::pair<
     // (rmsprop.py:169-172): 0, a negative value or None turns either clip off for this optimizer
     if (!(c.clip > 0.f)) c.clip = -1.f;
     if (!(c.clip_weights > 0.f)) c.clip_weights = -1.f;
+  }
+  if (c.kind == OPT_SIGNUM) {
+    // Signum.fused_step (signum.py:139-158): no state at momentum 0 -> signsgd_update; otherwise signum_update, handed
+    // the momentum only when it is > 0 (a negative momentum creates the state and runs the operator at momentum 0)
+    // and clip_gradient only when it is truthy (0, a negative value or None is off)
+    if (c.momentum == 0.f) c.kind = OPT_SIGNSGD;
+    if (!(c.momentum > 0.f)) c.momentum = 0.f;
+    if (!(c.clip > 0.f)) c.clip = -1.f;
   }
   if (c.kind == OPT_SGD && c.momentum != 0.f) c.kind = OPT_SGD_MOM;   // sgd.py:213-224
   if (c.kind == OPT_NAG && c.momentum == 0.f) c.kind = OPT_SGD;       // nag.py:59-63,141-154: no state, (mp_)sgd_update
@@ -578,6 +588,8 @@ float KVStore::KeyWD(const KeyState& ks) const {
   double wd = opt_.wd;
   auto it = opt_.wd_mult.find(ks.key);
   if (it != opt_.wd_mult.end()) wd *= it->second;
+  // signsgd_update is handed wd + wd_lh, summed in Python (double) and not multiplied by wd_mult (signum.py:156-158)
+  if (opt_.kind == OPT_SIGNSGD) wd += opt_.wd_lh;
   return static_cast<float>(wd);
 }
 
@@ -2220,6 +2232,7 @@ void KVStore::LaunchWorks(const LaunchClassKey& ck, std::vector<std::vector<Tens
     L.rescale = opt_.rescale; L.clip = opt_.clip; L.momentum = opt_.momentum;
     L.beta1 = static_cast<float>(opt_.beta1); L.beta2 = static_cast<float>(opt_.beta2); L.eps = opt_.eps;
     L.rho = opt_.rho; L.clip_weights = opt_.clip_weights;
+    L.wd_lh = static_cast<float>(opt_.wd_lh);
     L.sync.mode = ck.sync_mode;
     L.sync.world = n_part;
     L.sync.rank = p;

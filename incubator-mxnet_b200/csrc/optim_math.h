@@ -27,10 +27,16 @@ struct Hyper {
   float lr, wd, eta, rescale, clip, momentum, beta1, beta2, eps;
   bool mp;    // OPT_NAG only: MP_NAGMomKernel's grouping of the weight step (DenseLaunch::mp_arith)
   float rho, clip_weights;   // OPT_RMSPROP / OPT_RMSPROP_CENTERED (DenseLaunch::rho / clip_weights)
+  float wd_lh;               // OPT_SIGNUM (DenseLaunch::wd_lh)
 };
 
 MXKV_HD float clipf(float x, float b) {   // mshadow_op::clip, mshadow_op.h:999-1009
   return x > b ? b : (x < -b ? -b : x);
+}
+
+// (x > 0) - (x < 0) as the reference's Signum kernels write it: NaN and +-0 give 0
+MXKV_HD float signf(float x) {
+  return static_cast<float>((x > 0.0f) - (x < 0.0f));
 }
 
 // one element of the fused update; returns the new weight.  Operation order is
@@ -118,6 +124,19 @@ MXKV_HD float update_one(float g, float w, float& s0, float& s1, const Hyper& h)
     s0 = n;
     const float wn = __fsub_rn(w, __fdiv_rn(__fmul_rn(h.lr, r), __fadd_rn(__fsqrt_rn(n), h.eps)));
     return h.clip_weights >= 0.0f ? clipf(wn, h.clip_weights) : wn;
+  } else if (OPT == OPT_SIGNSGD) {
+    // SignSGDKernel: the sign of the summed gradient as it arrives -- rescale_grad and clip_gradient do not enter;
+    // wd is wd + wd_lh (KVStore::KeyWD).  lr * sign is exact.
+    return __fsub_rn(__fmul_rn(__fsub_rn(1.f, __fmul_rn(h.lr, h.wd)), w), __fmul_rn(h.lr, signf(g)));
+  } else if (OPT == OPT_SIGNUM) {
+    // SignumKernel (s0 = mom, the NEGATED average: the weight step is + lr * sign(mom))
+    float r = __fmul_rn(h.rescale, g);
+    if (h.clip >= 0.0f) r = clipf(r, h.clip);
+    r = __fadd_rn(r, __fmul_rn(h.wd, w));
+    float m = __fmul_rn(s0, h.momentum);
+    m = __fsub_rn(m, __fmul_rn(__fsub_rn(1.f, h.momentum), r));
+    s0 = m;
+    return __fadd_rn(__fmul_rn(__fsub_rn(1.f, __fmul_rn(h.lr, h.wd_lh)), w), __fmul_rn(h.lr, signf(m)));
   }
   return g;  // OPT_NONE
 }

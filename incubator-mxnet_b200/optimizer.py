@@ -1,9 +1,10 @@
-"""Optimizer descriptors mirroring python/mxnet/optimizer/{optimizer,sgd,nag,adam,adamW,adabelief,rmsprop,updater}.py.
+"""Optimizer descriptors mirroring python/mxnet/optimizer/{optimizer,sgd,nag,adam,adamW,adabelief,rmsprop,signum,
+updater}.py.
 
 Two roles:
 * describe the hyper-parameters of the optimizers that have a fused kernel in the native
-  engine (SGD / SGD-momentum / multi-precision SGD, NAG, Adam, AdamW, AdaBelief, RMSProp, Test, and the layer-wise adaptive
-  LAMB / LANS / LARS) -- ``KVStore.set_optimizer``
+  engine (SGD / SGD-momentum / multi-precision SGD, NAG, Adam, AdamW, AdaBelief, RMSProp, Signum, Test, and the
+  layer-wise adaptive LAMB / LANS / LARS) -- ``KVStore.set_optimizer``
   hands them to ``MXKVB200SetOptimizer`` and the update then runs inside the reduce kernel;
 * provide the generic ``Updater`` callback (updater.py:39-93) for any other Optimizer object:
   the store reduces on the GPU and calls back into Python, exactly like the reference.  The
@@ -441,6 +442,58 @@ class RMSProp(Optimizer):
                 w.clamp_(-self.clip_weights, self.clip_weights)
 
 
+def _sign(x):
+    """(x > 0) - (x < 0), as signum.py writes it: NaN gives 0 (torch.sign gives NaN)"""
+    return (x > 0).to(x.dtype) - (x < 0).to(x.dtype)
+
+
+@register
+class Signum(Optimizer):
+    """python/mxnet/optimizer/signum.py: signSGD / Signum (Bernstein et al., 2018); fused kernels signsgd_update
+    (no state, momentum 0) and signum_update (src/operator/optimizer_op-inl.h:2293-2379)::
+
+        momentum == 0:  weight = (1 - lr * (wd + wd_lh)) * weight - lr * sign(grad)
+        otherwise:      grad = clip(grad * rescale_grad, clip_gradient) + wd * weight
+                        mom = momentum * mom - (1 - momentum) * grad
+                        weight = (1 - lr * wd_lh) * weight + lr * sign(mom)
+
+    ``mom`` holds the negated average, as in the reference's state.  As in ``Signum.fused_step`` (signum.py:121-158),
+    the fused signsgd_update takes the sign of the raw summed gradient (rescale_grad and clip_gradient do not enter),
+    signum_update runs a negative momentum as 0, and a ``clip_gradient`` of 0, below 0 or None is off; ``wd_lh`` is
+    not multiplied by ``wd_mult``."""
+    fused_name = "signum"
+
+    def __init__(self, learning_rate=0.01, momentum=0.9, wd_lh=0.0, **kwargs):
+        super(Signum, self).__init__(learning_rate=learning_rate, **kwargs)
+        self.momentum, self.wd_lh = momentum, wd_lh
+
+    def fused_kwargs(self):
+        kw = super(Signum, self).fused_kwargs()
+        kw.update(momentum=self.momentum, wd_lh=self.wd_lh)
+        return kw
+
+    def create_state(self, index, weight):
+        import torch
+        return torch.zeros_like(weight.as_torch(), dtype=torch.float32) if self.momentum != 0.0 else None
+
+    def step(self, indices, weights, grads, states):     # signum.py:80-119
+        import torch
+        for index, weight, grad, state in zip(indices, weights, grads, states):
+            self._update_count(index)
+            lr = self._get_lr(index)
+            wd = self._get_wd(index)
+            w, g = weight.as_torch(), grad.as_torch().to(torch.float32)
+            if state is not None:
+                g = g * self.rescale_grad
+                if self.clip_gradient is not None:
+                    g = torch.clamp(g, -self.clip_gradient, self.clip_gradient)
+                g = g + wd * w
+                state.mul_(self.momentum).sub_((1 - self.momentum) * g)
+                w.mul_(1 - lr * self.wd_lh).add_(lr * _sign(state))
+            else:
+                w.mul_(1 - lr * (wd + self.wd_lh)).sub_(lr * _sign(g))
+
+
 class _LayerwiseAdaptive(Optimizer):
     """Shared part of LAMB / LANS / LARS: ``skip_nonfinite=True`` asks the store to leave weights and
     state alone when a merged gradient holds inf/nan (the AMP overflow skip, gluon/trainer.py:445-448,
@@ -641,8 +694,9 @@ class NativeUpdater(object):
     """Same call contract as :class:`Updater` (updater.py:39-93; ``index`` / ``grad`` / ``weight`` may be
     lists), but the whole list is updated IN PLACE by one fused launch (sequence) of the native engine
     -- what the reference does with ``multi_sgd_mom_update`` / ``multi_mp_sgd_*`` / ``multi_adamw`` /
-    ``multi_adabelief`` / ``rmsprop_update`` / ``multi_lamb`` / ``multi_lans`` when parameters are not updated on the kvstore (sgd.py:170-213,
-    lamb.py:170-215).  One instance serves one device, like ``Trainer._updaters[dev]``."""
+    ``multi_adabelief`` / ``rmsprop_update`` / ``signum_update`` / ``multi_lamb`` / ``multi_lans`` when parameters are
+    not updated on the kvstore (sgd.py:170-213, lamb.py:170-215).  One instance serves one device, like
+    ``Trainer._updaters[dev]``."""
 
     def __init__(self, optimizer):
         from . import kvstore as _kvs

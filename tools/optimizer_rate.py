@@ -3,7 +3,9 @@ the Python `step` (use_fused_step=False, the only way to run NAG before the fuse
 `--pair adabelief`: the fused AdaBelief against the fused Adam instead (both read g, w, mean, var and write stored w,
 mean, var, out: 32 bytes per float32 element).  With `--pair rmsprop`: the fused RMSProp against the fused SGD-momentum
 (24 bytes per float32 element each), the fused centered RMSProp against the fused Adam (40 against 32 bytes: it reads
-g, w, mean, var, mom and writes stored w, mean, var, mom, out), and RMSProp through the Python `step`.
+g, w, mean, var, mom and writes stored w, mean, var, mom, out), and RMSProp through the Python `step`.  With
+`--pair signum`: the fused Signum against the fused SGD-momentum (24 bytes per float32 element each), the fused
+signSGD against the fused SGD (16 bytes each: read g, w; write stored w, out), and Signum through the Python `step`.
 
 Two key sets: the bench sweep (9 float32 keys, 2^10 ... 2^26 elements) and ResNet-50's 193 gradient-carrying arrays
 (bench.py: keyset).  Both fused optimizers move the same bytes per element (read g, w, mom; write stored w, mom, out),
@@ -12,7 +14,7 @@ engine's stream (the Python path: host clock around a device synchronise, its to
 dense kernel variant that ran (launch counters), and one step checked against the CPU oracle.  The card's name and
 power limit are read with nvidia-smi in the same call and printed with the numbers.
 
-    python tools/optimizer_rate.py [--pair nag|adabelief|rmsprop] [--steps 200] [--warmup 20] [--rounds 3]
+    python tools/optimizer_rate.py [--pair nag|adabelief|rmsprop|signum] [--steps 200] [--warmup 20] [--rounds 3]
 """
 import argparse
 import ctypes
@@ -34,12 +36,14 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 KW = dict(learning_rate=0.01, momentum=0.9, wd=1e-4)
 KW_ADAPTIVE = dict(learning_rate=0.001, wd=1e-4)
 # --pair: (baseline, optimizer under test) pairs, alternated in one process; the python step is timed for the first
-# optimizer under test where it was the only way to run it (NAG, RMSProp)
+# optimizer under test where it was the only way to run it (NAG, RMSProp, Signum)
 PAIRS = {"nag": [("sgd", "nag")], "adabelief": [("adam", "adabelief")],
-         "rmsprop": [("sgd", "rmsprop"), ("adam", "rmsprop_centered")]}
-PYTHON_STEP = ("nag", "rmsprop")
+         "rmsprop": [("sgd", "rmsprop"), ("adam", "rmsprop_centered")],
+         "signum": [("sgd", "signum"), ("sgd_plain", "signsgd")]}
+PYTHON_STEP = ("nag", "rmsprop", "signum")
 LABELS = {"sgd": "sgd_momentum", "nag": "nag", "adam": "adam", "adabelief": "adabelief", "rmsprop": "rmsprop",
-          "rmsprop_centered": "rmsprop (centered)"}
+          "rmsprop_centered": "rmsprop (centered)", "sgd_plain": "sgd", "signum": "signum",
+          "signsgd": "signum (momentum 0: signsgd)"}
 VARIANTS = ("per_thread", "bulk", "nvls", "tree")
 
 
@@ -66,12 +70,15 @@ class Case(object):
         self.grads_np = [tile_fill(np.random.default_rng(1234 + k), -1, 1, s) for k, s in enumerate(shapes)]
         self.kv = mx.kv.create("device")
         self.kv.init(self.keys, [mx.nd.array(w, mx.gpu(0)) for w in w0])
-        self.kw = KW if optname in ("sgd", "nag") else KW_ADAPTIVE
+        self.kw = KW if optname in ("sgd", "nag", "signum") else KW_ADAPTIVE
         if optname.startswith("rmsprop"):
             self.kw = dict(KW_ADAPTIVE, centered=optname == "rmsprop_centered")
+        if optname in ("sgd_plain", "signsgd"):
+            self.kw = dict(KW, momentum=0.0)
         cls = {"sgd": mx.optimizer.SGD, "nag": mx.optimizer.NAG, "adam": mx.optimizer.Adam,
                "adabelief": mx.optimizer.AdaBelief, "rmsprop": mx.optimizer.RMSProp,
-               "rmsprop_centered": mx.optimizer.RMSProp}[optname]
+               "rmsprop_centered": mx.optimizer.RMSProp, "sgd_plain": mx.optimizer.SGD, "signum": mx.optimizer.Signum,
+               "signsgd": mx.optimizer.Signum}[optname]
         opt = cls(**dict(self.kw, **({} if fused else {"use_fused_step": False})))
         self.kv.set_optimizer(opt)
         self.grads = [mx.nd.array(g, mx.gpu(0)) for g in self.grads_np]
@@ -97,8 +104,11 @@ class Case(object):
         elif self.optname.startswith("rmsprop"):
             import rmsprop_oracle as R
             oopt = R.OracleRMSProp(**self.kw)
+        elif self.optname in ("signum", "signsgd"):
+            import signum_oracle as S
+            oopt = S.OracleSignum(**self.kw)
         else:
-            oopt = O.OracleOptimizer(self.optname, **self.kw)
+            oopt = O.OracleOptimizer("sgd" if self.optname == "sgd_plain" else self.optname, **self.kw)
         exact, close = True, True
         for k in self.keys:
             w = self.w0[k].reshape(-1).copy()
