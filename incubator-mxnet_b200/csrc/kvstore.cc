@@ -438,6 +438,7 @@ void KVStore::SetOptimizer(const std::string& name, const std::vector<std::pair<
   else if (n == "adabelief") { c.kind = OPT_ADABELIEF; c.lr = 0.001; c.eps = 1e-6f; }   // adabelief.py:79
   else if (n == "rmsprop") { c.kind = OPT_RMSPROP; c.lr = 0.001; c.momentum = 0.9f; }    // rmsprop.py:70-71
   else if (n == "signum") { c.kind = OPT_SIGNUM; c.lr = 0.01; c.momentum = 0.9f; }      // signum.py:67
+  else if (n == "ftml") { c.kind = OPT_FTML; c.lr = 0.0025; c.beta1 = 0.6; c.beta2 = 0.999; c.eps = 1e-8f; }  // ftml.py:66
   else MXKV_FATAL() << "optimizer '" << name << "' has no fused kernel; register a Python updater instead";
   for (auto& kv : kwargs) {
     const std::string& k = kv.first;
@@ -483,6 +484,9 @@ void KVStore::SetOptimizer(const std::string& name, const std::vector<std::pair<
     if (!(c.momentum > 0.f)) c.momentum = 0.f;
     if (!(c.clip > 0.f)) c.clip = -1.f;
   }
+  // FTML.fused_step hands clip_gradient to ftml_update only when it is truthy (ftml.py:152-153): 0, a negative value
+  // or None is off
+  if (c.kind == OPT_FTML && !(c.clip > 0.f)) c.clip = -1.f;
   if (c.kind == OPT_SGD && c.momentum != 0.f) c.kind = OPT_SGD_MOM;   // sgd.py:213-224
   if (c.kind == OPT_NAG && c.momentum == 0.f) c.kind = OPT_SGD;       // nag.py:59-63,141-154: no state, (mp_)sgd_update
   MXKV_CHECK(!c.skip_nonfinite || IsNormOpt(c.kind)) << "skip_nonfinite is available for lamb / lans / lars";
@@ -550,8 +554,18 @@ void KVStore::SetOptimizerMult(bool str_key, int ikey, const std::string& skey, 
 // have none).
 static bool EtaCarriesLR(int kind) { return kind == OPT_ADAMW || kind == OPT_ADABELIEF; }
 
+// FTML: the two powers of the update count t that FTMLKernel evaluates per element (optimizer_op-inl.h:1171-1172),
+// evaluated once per key as the operator's float arithmetic defines them -- t cast to float, beta^t, then
+// (1 - beta1^t) / lr in float with lr the float attribute Python hands over.  The powers are correctly rounded
+// (pow in double, rounded once), where the reference's device powf need not be.
+static float FtmlPow(double beta, int64_t count) {
+  const float t = static_cast<float>(count);
+  return static_cast<float>(std::pow(static_cast<double>(static_cast<float>(beta)), static_cast<double>(t)));
+}
+
 float KVStore::KeyLR(const KeyState& ks) const {
   if (EtaCarriesLR(opt_.kind)) return 1.0f;
+  if (opt_.kind == OPT_FTML) return (1.0f - FtmlPow(opt_.beta1, ks.count)) / static_cast<float>(KeyLRd(ks));
   return static_cast<float>(KeyLRd(ks));
 }
 
@@ -565,6 +579,7 @@ bool KVStore::SkipsOnRescale() const {
 
 float KVStore::KeyEta(const KeyState& ks) const {
   if (EtaCarriesLR(opt_.kind)) return static_cast<float>(KeyLRd(ks) * opt_.eta_d);
+  if (opt_.kind == OPT_FTML) return 1.0f - FtmlPow(opt_.beta2, ks.count);
   return opt_.eta;
 }
 

@@ -159,6 +159,20 @@ MXKV_HD float update_one(float g, float w, float& s0, float& s1, float& s2, cons
     s0 = m; s1 = n; s2 = d;
     const float wn = __fadd_rn(w, d);
     return h.clip_weights >= 0.0f ? clipf(wn, h.clip_weights) : wn;
+  } else if constexpr (OPT == OPT_FTML) {
+    // FTMLKernel (s0 = d, s1 = v, s2 = z).  The two powers of t arrive per key (KVStore::KeyLR / KeyEta):
+    // h.lr = (1 - beta1^t) / lr and h.eta = 1 - beta2^t, so that
+    //   v = beta2*v + (1-beta2)*r*r;  d_t = h.lr * (sqrt(v / h.eta) + eps)
+    //   z = (beta1*z + (1-beta1)*r) - (d_t - beta1*d)*w;  d = d_t;  w = -z / d_t
+    float r = __fmul_rn(h.rescale, g);
+    if (h.clip >= 0.0f) r = clipf(r, h.clip);
+    r = __fadd_rn(r, __fmul_rn(h.wd, w));
+    const float v = __fadd_rn(__fmul_rn(h.beta2, s1), __fmul_rn(__fsub_rn(1.f, h.beta2), __fmul_rn(r, r)));
+    const float dt = __fmul_rn(h.lr, __fadd_rn(__fsqrt_rn(__fdiv_rn(v, h.eta)), h.eps));
+    const float z = __fsub_rn(__fadd_rn(__fmul_rn(h.beta1, s2), __fmul_rn(__fsub_rn(1.f, h.beta1), r)),
+                              __fmul_rn(__fsub_rn(dt, __fmul_rn(h.beta1, s0)), w));
+    s0 = dt; s1 = v; s2 = z;
+    return __fdiv_rn(-z, dt);
   } else {
     return update_one<OPT>(g, w, s0, s1, h);
   }

@@ -100,8 +100,10 @@ kv_dense_tree_kernel(DenseLaunch L) {
   // 16-byte packets of float32, 8-byte packets (4 elements) of the 16-bit types: with three pending partial sums per
   // element next to a batch of loads, 8 elements per thread would not fit in the 64 registers that keep two blocks
   // of 512 threads resident (the residency the rendezvous grid is sized for)
-  // (float32 keys of centered RMSProp, with three state arrays, take one element at a time for the same reason)
-  constexpr int NV = sizeof(T) == 2 ? 4 : (OptHasS2(OPT) ? 1 : 16 / sizeof(T));
+  // (float32 keys of centered RMSProp and FTML, with three state arrays, take one element at a time for the same
+  // reason; so do FTML's 16-bit keys, which spill 32 / 48 bytes at 64 registers with 4-element packets)
+  constexpr int NV = (sizeof(T) == 2 && OPT == OPT_FTML) ? 1
+                   : (sizeof(T) == 2 ? 4 : (OptHasS2(OPT) ? 1 : 16 / sizeof(T)));
   const bool native_half_add = (sizeof(T) == 2) && !L.fp32_accum && (OPT == OPT_NONE);
   int cur = -1;
   for (int64_t c = blockIdx.x; c < L.total_chunks; c += gridDim.x) {

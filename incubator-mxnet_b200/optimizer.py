@@ -1,9 +1,9 @@
 """Optimizer descriptors mirroring python/mxnet/optimizer/{optimizer,sgd,nag,adam,adamW,adabelief,rmsprop,signum,
-updater}.py.
+ftml,updater}.py.
 
 Two roles:
 * describe the hyper-parameters of the optimizers that have a fused kernel in the native
-  engine (SGD / SGD-momentum / multi-precision SGD, NAG, Adam, AdamW, AdaBelief, RMSProp, Signum, Test, and the
+  engine (SGD / SGD-momentum / multi-precision SGD, NAG, Adam, AdamW, AdaBelief, RMSProp, Signum, FTML, Test, and the
   layer-wise adaptive LAMB / LANS / LARS) -- ``KVStore.set_optimizer``
   hands them to ``MXKVB200SetOptimizer`` and the update then runs inside the reduce kernel;
 * provide the generic ``Updater`` callback (updater.py:39-93) for any other Optimizer object:
@@ -492,6 +492,55 @@ class Signum(Optimizer):
                 w.mul_(1 - lr * self.wd_lh).add_(lr * _sign(state))
             else:
                 w.mul_(1 - lr * (wd + self.wd_lh)).sub_(lr * _sign(g))
+
+
+@register
+class FTML(Optimizer):
+    """python/mxnet/optimizer/ftml.py: Follow the Moving Leader (Zheng & Kwok, 2017); fused kernel ftml_update
+    (src/operator/optimizer_op-inl.h:1117-1206)::
+
+        grad = clip(grad * rescale_grad, clip_gradient) + wd * weight
+        v = beta2 * v + (1 - beta2) * grad**2
+        d_t = (1 - beta1**t) / lr * (sqrt(v / (1 - beta2**t)) + epsilon)
+        z = beta1 * z + (1 - beta1) * grad - (d_t - beta1 * d) * weight
+        d = d_t
+        weight = -z / d_t
+
+    As in ``FTML.fused_step`` (ftml.py:127-158), the fused update clips only where ``clip_gradient`` is truthy: 0, a
+    negative value or None is off (the non-fused ``step`` clips at 0)."""
+    fused_name = "ftml"
+
+    def __init__(self, learning_rate=0.0025, beta1=0.6, beta2=0.999, epsilon=1e-8, **kwargs):
+        super(FTML, self).__init__(learning_rate=learning_rate, **kwargs)
+        self.beta1, self.beta2, self.epsilon = beta1, beta2, epsilon
+
+    def fused_kwargs(self):
+        kw = super(FTML, self).fused_kwargs()
+        kw.update(beta1=self.beta1, beta2=self.beta2, epsilon=self.epsilon)
+        return kw
+
+    def create_state(self, index, weight):
+        import torch
+        w = weight.as_torch()
+        return tuple(torch.zeros_like(w, dtype=torch.float32) for _ in range(3))     # d, v, z
+
+    def step(self, indices, weights, grads, states):     # ftml.py:80-125
+        import torch
+        for index, weight, grad, state in zip(indices, weights, grads, states):
+            self._update_count(index)
+            lr = self._get_lr(index)
+            t = self._index_update_count[index]
+            w, g = weight.as_torch(), grad.as_torch()
+            g = _prep_grad(self, index, w, g)
+            coef1 = 1. - self.beta1 ** t
+            coef2 = 1. - self.beta2 ** t
+            d, v, z = state
+            v.mul_(self.beta2).add_((1. - self.beta2) * torch.square(g))
+            sigma = -self.beta1 * d
+            d.copy_(torch.sqrt(v / coef2) + self.epsilon).mul_(coef1 / lr)
+            sigma = sigma + d
+            z.mul_(self.beta1).add_((1. - self.beta1) * g).sub_(sigma * w)
+            w.copy_(-z / d)
 
 
 class _LayerwiseAdaptive(Optimizer):
