@@ -177,8 +177,8 @@ kv_dense_kernel(DenseLaunch L) {
 // One elected thread issues cp.async.bulk (the 1-D TMA path, SASS UBLKCP) for every input stream of
 // a tile -- the n gradient replicas (local HBM or NVLink peers), the weight and the optimizer state
 // -- into a ring of `stages` shared-memory buffers, arming an mbarrier with the byte count; all
-// threads wait on the barrier, compute the tile out of shared memory and store results straight
-// from registers.  Bytes in flight per SM are bounded by shared memory (up to ~200 KB) instead of by
+// threads wait on the barrier, take their operands of the tile into registers, release the stage for
+// the next request and then compute and store from registers.  Bytes in flight per SM are bounded by shared memory (up to ~200 KB) instead of by
 // registers (48 KB for the per-thread variant), which is what a latency-bound stream needs.
 // ---------------------------------------------------------------------------
 constexpr int kBulkThreads = 256;
@@ -188,6 +188,7 @@ constexpr int kBulkMaxStages = 8;
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t) { hostemu::MbarInit(bar); }
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) { hostemu::MbarExpectTx(bar, bytes); }
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) { hostemu::MbarWait(bar, parity); }
+__device__ __forceinline__ void fence_proxy_async() {}   // one memory on a CPU: bulk copies are plain memcpy
 __device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src_gmem, uint32_t bytes, uint64_t* bar) {
   hostemu::BulkCopy(dst_smem, src_gmem, bytes, bar);
 }
@@ -212,12 +213,25 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
       "DONE:\n\t"
       "}" :: "r"(smem_u32(bar)), "r"(parity) : "memory");
 }
+// orders this thread's generic-proxy accesses of shared memory before later async-proxy (bulk copy) accesses
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src_gmem, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                :: "r"(smem_u32(dst_smem)), "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
 
 #endif
+
+// Float4 columns of a tile a thread holds in registers between reading its stage and storing (the summed sources and
+// every staged fp32 stream of the kind, 4 + 4 * OptStreams floats each): 4 for kinds with at most one state array,
+// 2 for the wider ones, which keeps every instantiation within the 128 registers of two resident blocks.  A tile of up
+// to BulkMaxVecs * 4 * kBulkThreads elements is released before its stores.
+__host__ __device__ constexpr int BulkMaxVecs(int opt) { return OptStreams(opt) <= 2 ? 4 : 2; }
+
+__device__ __forceinline__ void ld_stage(const unsigned char* base, uint32_t arr_bytes, int a, int v, float (&x)[4]) {
+  const float4 t = reinterpret_cast<const float4*>(base + static_cast<size_t>(a) * arr_bytes)[v];
+  x[0] = t.x; x[1] = t.y; x[2] = t.z; x[3] = t.w;
+}
 
 template <int OPT, bool MP>
 __global__ void __launch_bounds__(kBulkThreads, 2)
@@ -240,6 +254,7 @@ kv_dense_bulk_kernel(DenseLaunch L) {
   constexpr bool HAS_S0 = OptHasS0(OPT);
   constexpr bool HAS_S1 = OptHasS1(OPT);
   constexpr bool HAS_S2 = OptHasS2(OPT);
+  constexpr int KV = BulkMaxVecs(OPT);
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < stages; ++s) mbar_init(&full[s], 1);
@@ -325,61 +340,81 @@ kv_dense_bulk_kernel(DenseLaunch L) {
     const unsigned char* base = bulk_smem + static_cast<size_t>(s) * stage_bytes;
     mbar_wait(&full[s], parity);
 
-    for (int v = threadIdx.x; v < nvec; v += blockDim.x) {
-      float acc[4], grp[4];
-      for (int k = 0; k < n; ++k) {
-        const float4 x4 = reinterpret_cast<const float4*>(base + static_cast<size_t>(k) * arr_bytes)[v];
-        const float x[4] = {x4.x, x4.y, x4.z, x4.w};
-        if (k == 0) {
+    // A thread takes its operands of up to KV float4 columns out of the stage into registers (the sources already
+    // summed), and the block releases the stage before anyone stores: the next tile's loads are then in flight during
+    // this tile's stores.  A tile wider than KV * blockDim columns is taken in passes; only the last one releases.
+    const int nthr = blockDim.x;
+    bool released = false;
+    for (int v0 = 0; v0 < nvec; v0 += KV * nthr) {
+      float acc[KV][4], w[KV][4], s0[KV][4], s1[KV][4], s2[KV][4];
 #pragma unroll
-          for (int j = 0; j < 4; ++j) acc[j] = x[j];
-        } else if (L.order == ORDER_DEVICE) {
+      for (int u = 0; u < KV; ++u) {
+        const int v = v0 + u * nthr + threadIdx.x;
+        if (v >= nvec) continue;
+        float grp[4];
+        for (int k = 0; k < n; ++k) {
+          const float4 x4 = reinterpret_cast<const float4*>(base + static_cast<size_t>(k) * arr_bytes)[v];
+          const float x[4] = {x4.x, x4.y, x4.z, x4.w};
+          if (k == 0) {
 #pragma unroll
-          for (int j = 0; j < 4; ++j) acc[j] = __fadd_rn(acc[j], x[j]);
-        } else {
-          const int pos = (k - 1) & 3;
+            for (int j = 0; j < 4; ++j) acc[u][j] = x[j];
+          } else if (L.order == ORDER_DEVICE) {
 #pragma unroll
-          for (int j = 0; j < 4; ++j) grp[j] = (pos == 0) ? x[j] : __fadd_rn(grp[j], x[j]);
-          if (pos == 3 || k == n - 1) {
+            for (int j = 0; j < 4; ++j) acc[u][j] = __fadd_rn(acc[u][j], x[j]);
+          } else {
+            const int pos = (k - 1) & 3;
 #pragma unroll
-            for (int j = 0; j < 4; ++j) acc[j] = __fadd_rn(acc[j], grp[j]);
+            for (int j = 0; j < 4; ++j) grp[j] = (pos == 0) ? x[j] : __fadd_rn(grp[j], x[j]);
+            if (pos == 3 || k == n - 1) {
+#pragma unroll
+              for (int j = 0; j < 4; ++j) acc[u][j] = __fadd_rn(acc[u][j], grp[j]);
+            }
           }
         }
+        if (OPT != OPT_NONE) {
+          int a = n;
+          ld_stage(base, arr_bytes, a++, v, w[u]);
+          if (HAS_S0) ld_stage(base, arr_bytes, a++, v, s0[u]);
+          if (HAS_S1) ld_stage(base, arr_bytes, a++, v, s1[u]);
+          if (HAS_S2) ld_stage(base, arr_bytes, a++, v, s2[u]);
+        }
       }
-      float wnew[4];
-      const int64_t e = cb + static_cast<int64_t>(v) * 4;
-      if (OPT == OPT_NONE) {
-#pragma unroll
-        for (int j = 0; j < 4; ++j) wnew[j] = acc[j];
-      } else {
-        int a = n;
-        const float4 w4 = reinterpret_cast<const float4*>(base + static_cast<size_t>(a) * arr_bytes)[v]; ++a;
-        float w[4] = {w4.x, w4.y, w4.z, w4.w};
-        float s0[4] = {0.f, 0.f, 0.f, 0.f}, s1[4] = {0.f, 0.f, 0.f, 0.f}, s2[4] = {0.f, 0.f, 0.f, 0.f};
-        if (HAS_S0) {
-          const float4 t4 = reinterpret_cast<const float4*>(base + static_cast<size_t>(a) * arr_bytes)[v]; ++a;
-          s0[0] = t4.x; s0[1] = t4.y; s0[2] = t4.z; s0[3] = t4.w;
-        }
-        if (HAS_S1) {
-          const float4 t4 = reinterpret_cast<const float4*>(base + static_cast<size_t>(a) * arr_bytes)[v]; ++a;
-          s1[0] = t4.x; s1[1] = t4.y; s1[2] = t4.z; s1[3] = t4.w;
-        }
-        if (HAS_S2) {
-          const float4 t4 = reinterpret_cast<const float4*>(base + static_cast<size_t>(a) * arr_bytes)[v]; ++a;
-          s2[0] = t4.x; s2[1] = t4.y; s2[2] = t4.z; s2[3] = t4.w;
-        }
-#pragma unroll
-        for (int j = 0; j < 4; ++j) wnew[j] = update_one<OPT>(acc[j], w[j], s0[j], s1[j], s2[j], h);
-        if (HAS_S0) stf<4>(tw.s0, e, s0);
-        if (HAS_S1) stf<4>(tw.s1, e, s1);
-        if (HAS_S2) stf<4>(tw.s2, e, s2);
-        if (MP) stf<4>(tw.w32, e, wnew);
+      if (v0 + KV * nthr >= nvec) {
+        // The stage's values are still in flight to registers here, and the refill is a write of the async proxy:
+        // without this fence it can overtake them.
+        fence_proxy_async();
+        __syncthreads();              // every thread is done reading stage s
+        released = true;
+        if (threadIdx.x == 0 && i + stages < ntiles) issue(i + stages);
       }
-      const int m = tw.n_out;
-      for (int j = 0; j < m; ++j) stf<4>(static_cast<float*>(tw.out[j]), e, wnew);
+#pragma unroll
+      for (int u = 0; u < KV; ++u) {
+        const int v = v0 + u * nthr + threadIdx.x;
+        if (v >= nvec) continue;
+        float wnew[4];
+        const int64_t e = cb + static_cast<int64_t>(v) * 4;
+        if (OPT == OPT_NONE) {
+#pragma unroll
+          for (int j = 0; j < 4; ++j) wnew[j] = acc[u][j];
+        } else {
+          if (!HAS_S0) { s0[u][0] = s0[u][1] = s0[u][2] = s0[u][3] = 0.f; }
+          if (!HAS_S1) { s1[u][0] = s1[u][1] = s1[u][2] = s1[u][3] = 0.f; }
+          if (!HAS_S2) { s2[u][0] = s2[u][1] = s2[u][2] = s2[u][3] = 0.f; }
+#pragma unroll
+          for (int j = 0; j < 4; ++j) wnew[j] = update_one<OPT>(acc[u][j], w[u][j], s0[u][j], s1[u][j], s2[u][j], h);
+          if (HAS_S0) stf<4>(tw.s0, e, s0[u]);
+          if (HAS_S1) stf<4>(tw.s1, e, s1[u]);
+          if (HAS_S2) stf<4>(tw.s2, e, s2[u]);
+          if (MP) stf<4>(tw.w32, e, wnew);
+        }
+        const int m = tw.n_out;
+        for (int j = 0; j < m; ++j) stf<4>(static_cast<float*>(tw.out[j]), e, wnew);
+      }
     }
-    __syncthreads();                  // every thread is done reading stage s
-    if (threadIdx.x == 0 && i + stages < ntiles) issue(i + stages);
+    if (!released) {
+      __syncthreads();
+      if (threadIdx.x == 0 && i + stages < ntiles) issue(i + stages);
+    }
   }
 
   if (sync) barrier_end(L.sync, L.sync.mode == SYNC_WRITE_PEERS);
@@ -717,7 +752,7 @@ static bool EnsureBulkAttr(int device, int opt, int multi_precision) {
 
 static int g_smem_budget = 0;   // MXKV_B200_BULK_SMEM_KB per block (default 100: two blocks per SM)
 
-int BulkPlan(int device, int opt, int multi_precision, int arrays, int* tile_elems, int* stages) {
+int BulkPlan(int device, int opt, int multi_precision, int arrays, bool local, int* tile_elems, int* stages) {
   BulkKernelFn fn = pick_bulk(opt, multi_precision);
   if (fn == nullptr || arrays < 1) return 0;
   if (g_smem_budget == 0) {
@@ -726,11 +761,14 @@ int BulkPlan(int device, int opt, int multi_precision, int arrays, int* tile_ele
     if (g_smem_budget < 16 * 1024) g_smem_budget = 16 * 1024;
     if (g_smem_budget > 200 * 1024) g_smem_budget = 200 * 1024;
   }
-  // 2048-element tiles, two stages (MXKV_B200_BULK_TILE / _STAGES override them): with two blocks per SM
-  // that is 2 x 100 KB of the 228 KB of shared memory an H100 SM has.  Wide work lists (many sources) fall
-  // back to 1024-element tiles to keep two blocks per SM resident.
-  int tile = 2048;
+  // Two stages (MXKV_B200_BULK_TILE / _STAGES override the geometry): with two blocks per SM that is 2 x 100 KB
+  // of the 228 KB of shared memory an H100 SM has.  A launch without a rendezvous takes the widest tile a thread
+  // releases before its stores (BulkMaxVecs: 4096 elements for kinds with at most one state array, 2048 for the
+  // others) that fits the budget; launches that read peers keep 2048, which is what was measured over NVLink.  Wide
+  // work lists (many sources) fall back to narrower tiles to keep two blocks per SM resident.
+  int tile = local ? BulkMaxVecs(opt) * 4 * kBulkThreads : 2048;
   int st = 2;
+  while (tile > 2048 && st * arrays * tile * 4 > g_smem_budget) tile /= 2;
   if (st * arrays * tile * 4 > g_smem_budget) tile = 1024;
   if (st * arrays * tile * 4 > g_smem_budget) return 0;
   {

@@ -211,8 +211,9 @@ int DenseMaxGrid(int device, int threads);   // resident-block capacity of the d
 int LaunchDenseTree(const DenseLaunch& L, cudaStream_t stream);
 int TreeKernelAvailable(int dtype, int opt, int multi_precision);
 // Plan the shared-memory staged variant for a float32 launch with `arrays` staged input streams per
-// tile: picks tile elements / stages and returns the resident grid capacity (0: not applicable).
-int BulkPlan(int device, int opt, int multi_precision, int arrays, int* tile_elems, int* stages);
+// tile: picks tile elements / stages and returns the resident grid capacity (0: not applicable).  `local`: the
+// launch has no rendezvous (SYNC_NONE), every stream is in this GPU's HBM.
+int BulkPlan(int device, int opt, int multi_precision, int arrays, bool local, int* tile_elems, int* stages);
 // Plan the multicast (NVLS) variant: elements per scheduling chunk (= one block iteration) for the given
 // requests-in-flight / pipelining / block size, and the resident grid capacity (0: not available).
 int NvlsPlan(int device, int opt, int multi_precision, int unroll, int pipe, int threads, int* chunk_elems);

@@ -2191,7 +2191,8 @@ void KVStore::LaunchWorks(const LaunchClassKey& ck, std::vector<std::vector<Tens
     if (ok && want) {
       // n_src is the same for every entry of a collective class; take the max for safety
       int tile = 0, st = 0;
-      const int cap = BulkPlan(part_dev[my_first], opt_kind, ck.mp, max_src + extra, &tile, &st);
+      const int cap = BulkPlan(part_dev[my_first], opt_kind, ck.mp, max_src + extra, ck.sync_mode == SYNC_NONE,
+                               &tile, &st);
       if (cap > 0) { bulk = 1; bulk_stages = st; bulk_arrays = max_src + extra; bulk_cap = cap; chunk = tile; }
     }
   }
@@ -2224,15 +2225,28 @@ void KVStore::LaunchWorks(const LaunchClassKey& ck, std::vector<std::vector<Tens
     const size_t wbytes = w.size() * sizeof(TensorWork);
     const size_t pbytes = prefix.size() * sizeof(int64_t);
     const size_t bytes = wbytes + pbytes;
-    const size_t off = d.ring.Alloc(bytes);
-    std::memcpy(d.ring.host(off), w.data(), wbytes);
-    std::memcpy(d.ring.host(off) + wbytes, prefix.data(), pbytes);
     DeviceGuard dg(dev);
-    CUDA_CALL(cudaMemcpyAsync(d.ring.dev(off), d.ring.host(off), bytes, cudaMemcpyHostToDevice, d.stream));
+    // The upload is a copy on the engine stream between two kernels, a fixed cost of every launch: a list that is
+    // byte-for-byte the resident one (the same keys pushed again with the same hyper-parameters) is read where it is.
+    // Any other list that fits replaces it, in stream order, so every kernel that reads the old list is done first.
+    const bool fits = bytes <= DeviceState::kResidentListBytes;
+    const bool resident = fits && d.list_host.size() == bytes &&
+                          std::memcmp(d.list_host.data(), w.data(), wbytes) == 0 &&
+                          std::memcmp(d.list_host.data() + wbytes, prefix.data(), pbytes) == 0;
+    size_t off = 0;
+    char* list = d.list_dev;
+    if (!resident) {
+      off = d.ring.Alloc(bytes);
+      std::memcpy(d.ring.host(off), w.data(), wbytes);
+      std::memcpy(d.ring.host(off) + wbytes, prefix.data(), pbytes);
+      if (!fits) list = d.ring.dev(off);
+      CUDA_CALL(cudaMemcpyAsync(list, d.ring.host(off), bytes, cudaMemcpyHostToDevice, d.stream));
+      if (fits) d.list_host.assign(d.ring.host(off), d.ring.host(off) + bytes);
+    }
     DenseLaunch L;
     std::memset(&L, 0, sizeof(L));
-    L.works = reinterpret_cast<const TensorWork*>(d.ring.dev(off));
-    L.chunk_prefix = reinterpret_cast<const int64_t*>(d.ring.dev(off) + wbytes);
+    L.works = reinterpret_cast<const TensorWork*>(list);
+    L.chunk_prefix = reinterpret_cast<const int64_t*>(list + wbytes);
     L.nworks = static_cast<int>(w.size());
     L.total_chunks = prefix.back();
     L.dtype = ck.dtype;
@@ -2275,7 +2289,7 @@ void KVStore::LaunchWorks(const LaunchClassKey& ck, std::vector<std::vector<Tens
     MXKV_CHECK(rc == 0) << "kernel launch failed: " << cudaGetErrorString(static_cast<cudaError_t>(rc));
     rt->launches++;
     rt->variant_launches[ck.tree ? 3 : (L.nvls ? 2 : (L.bulk ? 1 : 0))]++;
-    d.ring.Commit(off, bytes, d.stream);
+    if (!resident) d.ring.Commit(off, bytes, d.stream);
   }
 }
 

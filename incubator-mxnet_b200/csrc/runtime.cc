@@ -256,6 +256,7 @@ DeviceState& Runtime::Dev(int dev) {
     cudaGetLastError();
   }
   d->ring.Init(dev, static_cast<size_t>(EnvInt("MXKV_B200_RING_MB", 8)) << 20);
+  CUDA_CALL(cudaMalloc(reinterpret_cast<void**>(&d->list_dev), DeviceState::kResidentListBytes));
   d->max_grid = DenseMaxGrid(dev, threads);
   const int64_t cap = max_blocks_override_ > 0 ? max_blocks_override_ : EnvInt("MXKV_B200_MAX_BLOCKS", 0);
   if (cap > 0 && cap < d->max_grid) d->max_grid = static_cast<int>(cap);

@@ -19,6 +19,7 @@
 #include <memory>
 #include <mutex>
 #include <unordered_map>
+#include <vector>
 #include "base.h"
 
 namespace mxkv {
@@ -55,6 +56,11 @@ struct DeviceState {
   cudaEvent_t ev_xdev = nullptr;
   uint32_t* signal_pad = nullptr;      // this device's pad (SP mode: cudaMalloc; MP mode: in the arena)
   StagingRing ring;
+  // The dense work list (TensorWork[] + chunk prefix) last uploaded on `stream`, kept resident: a launch whose list is
+  // byte-for-byte the same (a pushpull of the same keys with the same hyper-parameters) reads it without an upload.
+  static constexpr size_t kResidentListBytes = 128 << 10;   // ResNet-50's and BERT-base's lists fit
+  char* list_dev = nullptr;
+  std::vector<char> list_host;         // what list_dev holds once the engine stream has reached this point
   int max_grid = 2 * kNumSms;
   bool engine_dirty = false;           // engine stream has work the user stream has not been fenced on
   // host-resident values: H2D / compute / D2H software pipeline (kvstore.cc: HostPipelined)
