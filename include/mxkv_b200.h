@@ -143,8 +143,8 @@ MXKV_DLL int MXKVStoreSendCommmandToServers(KVStoreHandle handle, int cmd_id, co
 /* ---- MXKVB200 extensions -------------------------------------------------- */
 /* Fused optimizer: what Python's Updater + sgd_update/adam_update ops do per key in the
  * reference (python/mxnet/optimizer/updater.py:39-93) happens inside the reduce kernel.
- * name: "sgd" | "nag" | "adam" | "adamw" | "adabelief" | "rmsprop" | "signum" | "ftml" | "test" | "lamb" | "lans" |
- * "lars";
+ * name: "sgd" | "nag" | "adam" | "adamw" | "adabelief" | "rmsprop" | "signum" | "ftml" | "adamax" | "adadelta" |
+ * "test" | "lamb" | "lans" | "lars";
  * kwargs use the reference's hyper-parameter names (learning_rate, wd, momentum, rescale_grad, clip_gradient, beta1,
  * beta2, epsilon, eta, multi_precision, lazy_update, correct_bias, lower_bound, upper_bound,
  * bias_correction, rho, centered, clip_weights, wd_lh).  rmsprop: centered=True selects rmspropalex_update; a
@@ -153,7 +153,11 @@ MXKV_DLL int MXKVStoreSendCommmandToServers(KVStoreHandle handle, int cmd_id, co
  * + wd_lh as its weight decay, rescale_grad and clip_gradient unused), any other momentum signum_update (a negative
  * one runs it at momentum 0); clip_gradient is off at 0, below 0 or None, as for rmsprop.  ftml: ftml_update with
  * the class defaults learning_rate 0.0025, beta1 0.6, beta2 0.999, epsilon 1e-8; clip_gradient is off at 0, below 0
- * or None, as FTML.fused_step passes it only when it is truthy.  lamb / lans / lars
+ * or None, as FTML.fused_step passes it only when it is truthy.  adamax / adadelta: Adamax.step / AdaDelta.step
+ * restated (the reference has no operator for either), every scalar parsed as a double and rounded once to float, as
+ * Python hands it to an NDArray operation; class defaults learning_rate 0.002, beta1 0.9, beta2 0.999, epsilon 1e-8
+ * (adamax) and learning_rate 1.0, rho 0.9, epsilon 1e-6 (adadelta); clip_gradient clips at 0 too, as step does, and
+ * is off below 0 or None.  lamb / lans / lars
  * additionally take skip_nonfinite=True: when any merged gradient of a push holds inf/nan, that push changes neither
  * weights nor optimizer state (the AMP overflow skip of gluon/trainer.py:445-448, decided on the device inside the
  * same launch sequence). */
@@ -168,7 +172,8 @@ MXKV_DLL int MXKVB200SetOptimizerMult(KVStoreHandle handle, int key, const char*
  * kvstore (multi_sgd_update / multi_sgd_mom_update / multi_mp_sgd_*, src/operator/optimizer_op-inl.h:
  * 207-375; nag_mom_update / mp_nag_mom_update per weight, :1029-1092; multi_adamw, multi_adabelief,
  * multi_lamb, multi_lans; rmsprop_update / rmspropalex_update per weight, :1905-2031; signsgd_update /
- * signum_update per weight, :2293-2379; ftml_update per weight, :1117-1206).  Create the handle with MXKVStoreCreate("updater"), give it an optimizer with MXKVB200SetOptimizer, then every call updates all (weight, grad) pairs
+ * signum_update per weight, :2293-2379; ftml_update per weight, :1117-1206; Adamax.step / AdaDelta.step, which have
+ * no operator).  Create the handle with MXKVStoreCreate("updater"), give it an optimizer with MXKVB200SetOptimizer, then every call updates all (weight, grad) pairs
  * IN PLACE with one launch (sequence) on their GPU.  Optimizer state of an index is created on first
  * sight and is reachable through MXKVB200GetState / SetState / Get|SetUpdateCount.  One handle serves
  * one device, like the reference's `Trainer._updaters[dev]`.  Never collective.  grads == NULL only
@@ -181,7 +186,9 @@ MXKV_DLL int MXKVB200UpdaterStepEx(KVStoreHandle handle, uint32_t num, const cha
  * (learning rate with lr_mult and, for Adam, the host-side bias correction folded in; weight decay with
  * wd_mult; AdamW and AdaBelief: operator lr = 1 and eta = the bias-corrected learning rate; FTML: lr =
  * (1 - beta1^t) / (learning rate x lr_mult) and eta = 1 - beta2^t, the two powers of the update count t that
- * ftml_update takes per element, in float as the operator does).  Host-only, no GPU needed. */
+ * ftml_update takes per element, in float as the operator does; Adamax: lr = learning rate x lr_mult / (1 - beta1^t)
+ * and eta = 1 - beta1; AdaDelta: eta = 1 - rho -- each computed in double and rounded once).  Host-only, no GPU
+ * needed. */
 MXKV_DLL int MXKVB200GetKeyHyper(KVStoreHandle handle, int key, const char* str_key, float* lr, float* wd,
                                  float* eta);
 /* per-key switch of a fused optimizer.  "no_trust_ratio" != 0: LARS keeps the plain learning rate
@@ -198,8 +205,9 @@ MXKV_DLL int MXKVB200GetOverflow(KVStoreHandle handle, int* out);
 MXKV_DLL int MXKVB200MultiSumSq(uint32_t num, NDArrayHandle* arrays, float scale, NDArrayHandle out);
 MXKV_DLL int MXKVB200MultiAllFinite(uint32_t num, NDArrayHandle* arrays, int init_output, NDArrayHandle out);
 /* which: 0 stored value, 1 fp32 master weight, 2 state0 (momentum | mean | RMSProp var; centered RMSProp: mean;
- * Signum: the negated momentum, as the reference stores it; FTML: d),
- * 3 state1 (variance; FTML: v), 4 state2 (centered RMSProp momentum; FTML: z).
+ * Signum: the negated momentum, as the reference stores it; FTML: d; Adamax: mean; AdaDelta: acc_g),
+ * 3 state1 (variance; FTML: v; Adamax: var, the max-norm; AdaDelta: acc_delta), 4 state2 (centered RMSProp momentum;
+ * FTML: z).
  * Returns a NEW handle aliasing engine memory (free it with MXNDArrayFree); *out = NULL when the
  * state does not exist. */
 MXKV_DLL int MXKVB200GetState(KVStoreHandle handle, int key, const char* str_key, int which,

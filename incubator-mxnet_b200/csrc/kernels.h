@@ -47,24 +47,28 @@ enum OptKind : int {
   OPT_RMSPROP_CENTERED = 14, // RMSPropAlexUpdateKernel      optimizer_op-inl.h:1905-1939
   OPT_SIGNSGD = 15,   // SignSGDKernel                       optimizer_op-inl.h:2293-2305
   OPT_SIGNUM = 16,    // SignumKernel                        optimizer_op-inl.h:2361-2379
-  OPT_FTML = 17       // FTMLKernel                          optimizer_op-inl.h:1159-1177
+  OPT_FTML = 17,      // FTMLKernel                          optimizer_op-inl.h:1159-1177
+  // no reference operator: the optimizer class's own `step`, one NDArray operation per rounding
+  OPT_ADAMAX = 18,    // Adamax.step                         python/mxnet/optimizer/adamax.py:74-111
+  OPT_ADADELTA = 19   // AdaDelta.step                       python/mxnet/optimizer/adadelta.py:72-111
 };
-constexpr int kNumOptKinds = OPT_FTML + 1;   // one past the last kind: the size of tables indexed by kind
+constexpr int kNumOptKinds = OPT_ADADELTA + 1;   // one past the last kind: the size of tables indexed by kind
 inline bool IsNormOpt(int kind) { return kind == OPT_LAMB || kind == OPT_LANS || kind == OPT_LARS; }
 
 // The fp32 state arrays an element-wise kind streams through update_one: s0 (momentum / mean / RMSProp var;
-// centered RMSProp: mean; Signum: the negated momentum; FTML: d), s1 (variance; FTML: v), s2 (centered RMSProp:
-// momentum; FTML: z) -- the tuple order of the reference's create_state.  Every dense kernel loads and stores exactly
+// centered RMSProp: mean; Signum: the negated momentum; FTML: d; Adamax: mean; AdaDelta: acc_g), s1 (variance; FTML:
+// v; Adamax: the max-norm u; AdaDelta: acc_delta), s2 (centered RMSProp: momentum; FTML: z) -- the tuple order of the
+// reference's create_state.  Every dense kernel loads and stores exactly
 // these, and the staged kernel counts them among its staged arrays.  The layer-wise adaptive kinds keep their state
 // rules with their launch sequence (KVStore::EnsureState).
 __host__ __device__ constexpr bool OptHasS0(int kind) {
   return kind == OPT_SGD_MOM || kind == OPT_ADAM || kind == OPT_ADAMW || kind == OPT_ADAM_STD || kind == OPT_NAG ||
          kind == OPT_ADABELIEF || kind == OPT_RMSPROP || kind == OPT_RMSPROP_CENTERED || kind == OPT_SIGNUM ||
-         kind == OPT_FTML;
+         kind == OPT_FTML || kind == OPT_ADAMAX || kind == OPT_ADADELTA;
 }
 __host__ __device__ constexpr bool OptHasS1(int kind) {
   return kind == OPT_ADAM || kind == OPT_ADAMW || kind == OPT_ADAM_STD || kind == OPT_ADABELIEF ||
-         kind == OPT_RMSPROP_CENTERED || kind == OPT_FTML;
+         kind == OPT_RMSPROP_CENTERED || kind == OPT_FTML || kind == OPT_ADAMAX || kind == OPT_ADADELTA;
 }
 __host__ __device__ constexpr bool OptHasS2(int kind) { return kind == OPT_RMSPROP_CENTERED || kind == OPT_FTML; }
 // The fp32 arrays a kind streams next to its gradients: the weight (every kind but OPT_NONE) and its state arrays.
@@ -92,7 +96,8 @@ struct OptKinds {
   }
 };
 using ElementwiseOpts = OptKinds<OPT_SGD, OPT_SGD_MOM, OPT_ADAM, OPT_ADAMW, OPT_TEST, OPT_NAG, OPT_ADABELIEF,
-                                 OPT_RMSPROP, OPT_RMSPROP_CENTERED, OPT_SIGNSGD, OPT_SIGNUM, OPT_FTML>;
+                                 OPT_RMSPROP, OPT_RMSPROP_CENTERED, OPT_SIGNSGD, OPT_SIGNUM, OPT_FTML, OPT_ADAMAX,
+                                 OPT_ADADELTA>;
 
 enum SumOrder : int {
   ORDER_DEVICE = 0,  // ((in0+in1)+in2)+...                  ndarray_function-inl.h:457-486
@@ -116,9 +121,10 @@ struct alignas(16) TensorWork {
   float* s1;         // adam variance
   int64_t begin;     // element range [begin, end) of the key handled by this launch
   int64_t end;
-  float lr;          // per-key learning rate (lr_mult, scheduler, Adam bias correction folded in; FTML: (1-beta1^t)/lr)
+  float lr;          // per-key learning rate (lr_mult, scheduler, Adam / Adamax bias correction folded in; FTML:
+                     //   (1-beta1^t)/lr)
   float wd;          // per-key weight decay
-  float eta;         // AdamW schedule multiplier (FTML: 1 - beta2^t)
+  float eta;         // AdamW schedule multiplier (FTML: 1 - beta2^t; Adamax: 1 - beta1, AdaDelta: 1 - rho, in double)
   int n_src;
   int n_out;
   int flags;         // kWork* bits (WorkFlags)

@@ -439,7 +439,20 @@ void KVStore::SetOptimizer(const std::string& name, const std::vector<std::pair<
   else if (n == "rmsprop") { c.kind = OPT_RMSPROP; c.lr = 0.001; c.momentum = 0.9f; }    // rmsprop.py:70-71
   else if (n == "signum") { c.kind = OPT_SIGNUM; c.lr = 0.01; c.momentum = 0.9f; }      // signum.py:67
   else if (n == "ftml") { c.kind = OPT_FTML; c.lr = 0.0025; c.beta1 = 0.6; c.beta2 = 0.999; c.eps = 1e-8f; }  // ftml.py:66
+  // adamax.py:61, adadelta.py:62.  Both keep the generic clip rule: `step` clips whenever clip_gradient is not None,
+  // at 0 too.  A negative bound is off here, where `step` would clip to the inverted interval [-c, c]
+  else if (n == "adamax") {
+    c.kind = OPT_ADAMAX; c.lr = 0.002; c.beta1 = 0.9; c.beta2 = 0.999; c.eps = static_cast<float>(1e-8);
+  } else if (n == "adadelta") {
+    c.kind = OPT_ADADELTA; c.lr = 1.0; c.rho_d = 0.9; c.rho = static_cast<float>(0.9); c.eps = static_cast<float>(1e-6);
+  }
   else MXKV_FATAL() << "optimizer '" << name << "' has no fused kernel; register a Python updater instead";
+  // Adamax and AdaDelta restate their optimizer's Python `step`, where a scalar enters an NDArray operation as
+  // float32(double): parse as double, then round once (std::stof may round the decimal string differently)
+  const bool from_double = c.kind == OPT_ADAMAX || c.kind == OPT_ADADELTA;
+  auto to_float = [from_double](const std::string& v) {
+    return from_double ? static_cast<float>(std::stod(v)) : std::stof(v);
+  };
   for (auto& kv : kwargs) {
     const std::string& k = kv.first;
     const std::string& v = kv.second;
@@ -448,7 +461,7 @@ void KVStore::SetOptimizer(const std::string& name, const std::vector<std::pair<
     else if (k == "momentum") c.momentum = std::stof(v);
     else if (k == "beta1") c.beta1 = std::stod(v);
     else if (k == "beta2") c.beta2 = std::stod(v);
-    else if (k == "epsilon") { if (c.kind == OPT_LARS) c.lars_eps = std::stof(v); else c.eps = std::stof(v); }
+    else if (k == "epsilon") { if (c.kind == OPT_LARS) c.lars_eps = std::stof(v); else c.eps = to_float(v); }
     else if (k == "eta") {
       if (c.kind == OPT_LARS) c.lars_eta = std::stof(v);
       else { c.eta = std::stof(v); c.eta_d = std::stod(v); }
@@ -457,13 +470,13 @@ void KVStore::SetOptimizer(const std::string& name, const std::vector<std::pair<
     else if (k == "upper_bound") c.upper_bound = (v == "None" || v.empty()) ? -1.f : std::stof(v);
     else if (k == "bias_correction") c.bias_correction = (v == "True" || v == "true" || v == "1");
     else if (k == "skip_nonfinite") c.skip_nonfinite = (v == "True" || v == "true" || v == "1");
-    else if (k == "rescale_grad") c.rescale = std::stof(v);
-    else if (k == "clip_gradient") c.clip = (v == "None" || v.empty()) ? -1.f : std::stof(v);
+    else if (k == "rescale_grad") c.rescale = to_float(v);
+    else if (k == "clip_gradient") c.clip = (v == "None" || v.empty()) ? -1.f : to_float(v);
     else if (k == "lazy_update") c.lazy_update = (v == "True" || v == "true" || v == "1");
     else if (k == "correct_bias") c.correct_bias = (v == "True" || v == "true" || v == "1");
     else if (k == "multi_precision") c.multi_precision = (v == "True" || v == "true" || v == "1");
     else if (k == "reset_states") reset_states = (v == "True" || v == "true" || v == "1");
-    else if (k == "rho") c.rho = std::stof(v);
+    else if (k == "rho") { c.rho = to_float(v); c.rho_d = std::stod(v); }
     else if (k == "centered") centered = (v == "True" || v == "true" || v == "1");
     else if (k == "clip_weights") c.clip_weights = (v == "None" || v.empty()) ? -1.f : std::stof(v);
     else if (k == "wd_lh") c.wd_lh = std::stod(v);
@@ -563,6 +576,11 @@ static float FtmlPow(double beta, int64_t count) {
   return static_cast<float>(std::pow(static_cast<double>(static_cast<float>(beta)), static_cast<double>(t)));
 }
 
+// Adamax and AdaDelta: the complement that `step` writes as `(1. - beta1) * grad` / `(1. - rho) * square(...)` --
+// computed in double, then rounded once.  1.f - float(beta1) is a different number for most betas (0.1f against
+// 0.100000024f at beta1 = 0.9)
+static bool EtaIsComplement(int kind) { return kind == OPT_ADAMAX || kind == OPT_ADADELTA; }
+
 float KVStore::KeyLR(const KeyState& ks) const {
   if (EtaCarriesLR(opt_.kind)) return 1.0f;
   if (opt_.kind == OPT_FTML) return (1.0f - FtmlPow(opt_.beta1, ks.count)) / static_cast<float>(KeyLRd(ks));
@@ -580,6 +598,7 @@ bool KVStore::SkipsOnRescale() const {
 float KVStore::KeyEta(const KeyState& ks) const {
   if (EtaCarriesLR(opt_.kind)) return static_cast<float>(KeyLRd(ks) * opt_.eta_d);
   if (opt_.kind == OPT_FTML) return 1.0f - FtmlPow(opt_.beta2, ks.count);
+  if (EtaIsComplement(opt_.kind)) return static_cast<float>(1.0 - (opt_.kind == OPT_ADAMAX ? opt_.beta1 : opt_.rho_d));
   return opt_.eta;
 }
 
@@ -596,6 +615,8 @@ double KVStore::KeyLRd(const KeyState& ks) const {
     const double coef2 = 1. - std::pow(opt_.beta2, t);
     lr *= std::sqrt(coef2) / coef1;
   }
+  // adamax.py:93: lr /= (1. - self.beta1**t)
+  if (opt_.kind == OPT_ADAMAX) lr /= (1. - std::pow(opt_.beta1, static_cast<double>(ks.count)));
   return lr;
 }
 

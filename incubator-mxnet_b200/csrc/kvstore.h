@@ -42,6 +42,7 @@ struct OptimizerConfig {
   bool lazy_update = false;   // row_sparse gradients: touch only the rows present (sgd.py:78, adam.py:77 default False)
   bool correct_bias = true;   // AdamW, AdaBelief (python/mxnet/optimizer/adamW.py:80-88, adabelief.py:79-87)
   float rho = 0.9f, clip_weights = -1.f;   // RMSProp (rmsprop.py:70-71); clip_weights < 0: off
+  double rho_d = 0.9;         // rho as given (AdaDelta's 1 - rho is computed in double)
   double wd_lh = 0.0;         // Signum's decoupled weight decay (signum.py:67); double: signSGD adds it to wd in double
   // LAMB / LANS / LARS (python/mxnet/optimizer/{lamb,lans,lars}.py)
   float lower_bound = -1.f, upper_bound = -1.f;   // bounds on the weight norm, < 0: not set

@@ -39,6 +39,12 @@ MXKV_HD float signf(float x) {
   return static_cast<float>((x > 0.0f) - (x < 0.0f));
 }
 
+// mshadow_op::maximum (mshadow_op.h:1266-1275): a NaN in either operand gives NaN -- unlike fmaxf, which returns the
+// other operand
+MXKV_HD float maximumf(float a, float b) {
+  return a != a ? a : (a > b ? a : b);
+}
+
 // one element of the fused update; returns the new weight.  Operation order is
 // the reference source's, see the OptKind comments in kernels.h.
 template <int OPT>
@@ -137,6 +143,30 @@ MXKV_HD float update_one(float g, float w, float& s0, float& s1, const Hyper& h)
     m = __fsub_rn(m, __fmul_rn(__fsub_rn(1.f, h.momentum), r));
     s0 = m;
     return __fadd_rn(__fmul_rn(__fsub_rn(1.f, __fmul_rn(h.lr, h.wd_lh)), w), __fmul_rn(h.lr, signf(m)));
+  } else if (OPT == OPT_ADAMAX) {
+    // Adamax.step (s0 = mean, s1 = var, the max-norm u), one NDArray operation per rounding.  Per key (KVStore::KeyLR /
+    // KeyEta): h.lr = lr / (1 - beta1^t) and h.eta = 1 - beta1, each computed in double and rounded once, as Python
+    // hands a scalar to an NDArray operation
+    float r = __fmul_rn(g, h.rescale);
+    if (h.clip >= 0.0f) r = clipf(r, h.clip);
+    r = __fadd_rn(r, __fmul_rn(h.wd, w));
+    const float m = __fadd_rn(__fmul_rn(s0, h.beta1), __fmul_rn(h.eta, r));
+    const float u = maximumf(__fmul_rn(h.beta2, s1), fabsf(r));
+    s0 = m; s1 = u;
+    return __fsub_rn(w, __fmul_rn(h.lr, __fdiv_rn(m, __fadd_rn(u, h.eps))));
+  } else if (OPT == OPT_ADADELTA) {
+    // AdaDelta.step (s0 = acc_g, s1 = acc_delta), one NDArray operation per rounding; h.eta = 1 - rho computed in
+    // double and rounded once (KVStore::KeyEta).  The step size is taken from the OLD acc_delta
+    float r = __fmul_rn(g, h.rescale);
+    if (h.clip >= 0.0f) r = clipf(r, h.clip);
+    r = __fadd_rn(r, __fmul_rn(h.wd, w));
+    const float ag = __fadd_rn(__fmul_rn(s0, h.rho), __fmul_rn(h.eta, __fmul_rn(r, r)));
+    float cd = __fsqrt_rn(__fadd_rn(s1, h.eps));
+    cd = __fdiv_rn(cd, __fsqrt_rn(__fadd_rn(ag, h.eps)));
+    cd = __fmul_rn(cd, r);
+    const float ad = __fadd_rn(__fmul_rn(s1, h.rho), __fmul_rn(h.eta, __fmul_rn(cd, cd)));
+    s0 = ag; s1 = ad;
+    return __fsub_rn(w, __fmul_rn(h.lr, cd));
   }
   return g;  // OPT_NONE
 }

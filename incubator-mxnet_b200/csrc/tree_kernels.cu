@@ -101,9 +101,11 @@ kv_dense_tree_kernel(DenseLaunch L) {
   // element next to a batch of loads, 8 elements per thread would not fit in the 64 registers that keep two blocks
   // of 512 threads resident (the residency the rendezvous grid is sized for)
   // (float32 keys of centered RMSProp and FTML, with three state arrays, take one element at a time for the same
-  // reason; so do FTML's 16-bit keys, which spill 32 / 48 bytes at 64 registers with 4-element packets)
+  // reason; so do FTML's 16-bit keys, which spill 32 / 48 bytes at 64 registers with 4-element packets, and the
+  // float32 keys of Adamax and AdaDelta, which spill 12 / 16 bytes with them)
+  constexpr bool kOneElem = OPT == OPT_ADAMAX || OPT == OPT_ADADELTA;
   constexpr int NV = (sizeof(T) == 2 && OPT == OPT_FTML) ? 1
-                   : (sizeof(T) == 2 ? 4 : (OptHasS2(OPT) ? 1 : 16 / sizeof(T)));
+                   : (sizeof(T) == 2 ? 4 : ((OptHasS2(OPT) || kOneElem) ? 1 : 16 / sizeof(T)));
   const bool native_half_add = (sizeof(T) == 2) && !L.fp32_accum && (OPT == OPT_NONE);
   int cur = -1;
   for (int64_t c = blockIdx.x; c < L.total_chunks; c += gridDim.x) {

@@ -1,10 +1,10 @@
 """Optimizer descriptors mirroring python/mxnet/optimizer/{optimizer,sgd,nag,adam,adamW,adabelief,rmsprop,signum,
-ftml,updater}.py.
+ftml,adamax,adadelta,updater}.py.
 
 Two roles:
 * describe the hyper-parameters of the optimizers that have a fused kernel in the native
-  engine (SGD / SGD-momentum / multi-precision SGD, NAG, Adam, AdamW, AdaBelief, RMSProp, Signum, FTML, Test, and the
-  layer-wise adaptive LAMB / LANS / LARS) -- ``KVStore.set_optimizer``
+  engine (SGD / SGD-momentum / multi-precision SGD, NAG, Adam, AdamW, AdaBelief, RMSProp, Signum, FTML, Adamax,
+  AdaDelta, Test, and the layer-wise adaptive LAMB / LANS / LARS) -- ``KVStore.set_optimizer``
   hands them to ``MXKVB200SetOptimizer`` and the update then runs inside the reduce kernel;
 * provide the generic ``Updater`` callback (updater.py:39-93) for any other Optimizer object:
   the store reduces on the GPU and calls back into Python, exactly like the reference.  The
@@ -543,6 +543,98 @@ class FTML(Optimizer):
             w.copy_(-z / d)
 
 
+def _maximum(a, b):
+    """mshadow_op::maximum (mshadow_op.h:1266-1275): NaN in either operand gives NaN, as torch.maximum does"""
+    import torch
+    return torch.maximum(a, b)
+
+
+@register
+class Adamax(Optimizer):
+    """python/mxnet/optimizer/adamax.py: AdaMax, the infinity-norm variant of Adam (Kingma & Ba, 2014, section 7).
+    The reference has no operator for it: the fused kernel restates ``Adamax.step`` (adamax.py:74-111) one float32
+    operation per NDArray operation, every Python scalar rounded once from its double::
+
+        grad = clip(grad * rescale_grad, clip_gradient) + wd * weight
+        mean = beta1 * mean + (1 - beta1) * grad
+        var = maximum(beta2 * var, abs(grad))
+        weight = weight - lr / (1 - beta1**t) * (mean / (var + epsilon))
+
+    ``clip_gradient`` clips whenever it is not None, at 0 too; a negative one is off in the fused kernel."""
+    fused_name = "adamax"
+
+    def __init__(self, learning_rate=0.002, beta1=0.9, beta2=0.999, epsilon=1e-8, **kwargs):
+        super(Adamax, self).__init__(learning_rate=learning_rate, **kwargs)
+        self.beta1, self.beta2, self.epsilon = beta1, beta2, epsilon
+
+    def fused_kwargs(self):
+        kw = super(Adamax, self).fused_kwargs()
+        kw.update(beta1=self.beta1, beta2=self.beta2, epsilon=self.epsilon)
+        return kw
+
+    def create_state(self, index, weight):
+        import torch
+        w = weight.as_torch()
+        return tuple(torch.zeros_like(w, dtype=torch.float32) for _ in range(2))     # mean, var
+
+    def step(self, indices, weights, grads, states):     # adamax.py:74-111
+        for index, weight, grad, state in zip(indices, weights, grads, states):
+            self._update_count(index)
+            lr = self._get_lr(index)
+            t = self._index_update_count[index]
+            lr /= (1. - self.beta1 ** t)
+            w, g = weight.as_torch(), grad.as_torch()
+            g = _prep_grad(self, index, w, g)
+            mean, var = state
+            mean.mul_(self.beta1).add_((1. - self.beta1) * g)
+            var.copy_(_maximum(self.beta2 * var, g.abs()))
+            w.sub_(lr * (mean / (var + self.epsilon)))
+
+
+@register
+class AdaDelta(Optimizer):
+    """python/mxnet/optimizer/adadelta.py: AdaDelta (Zeiler, 2012).  The reference has no operator for it: the fused
+    kernel restates ``AdaDelta.step`` (adadelta.py:72-111) one float32 operation per NDArray operation, every Python
+    scalar rounded once from its double::
+
+        grad = clip(grad * rescale_grad, clip_gradient) + wd * weight
+        acc_g = rho * acc_g + (1 - rho) * grad**2
+        delta = sqrt(acc_delta + epsilon) / sqrt(acc_g + epsilon) * grad
+        acc_delta = rho * acc_delta + (1 - rho) * delta**2
+        weight = weight - lr * delta
+
+    ``clip_gradient`` clips whenever it is not None, at 0 too; a negative one is off in the fused kernel."""
+    fused_name = "adadelta"
+
+    def __init__(self, learning_rate=1.0, rho=0.9, epsilon=1e-6, **kwargs):
+        super(AdaDelta, self).__init__(learning_rate=learning_rate, **kwargs)
+        self.rho, self.epsilon = rho, epsilon
+
+    def fused_kwargs(self):
+        kw = super(AdaDelta, self).fused_kwargs()
+        kw.update(rho=self.rho, epsilon=self.epsilon)
+        return kw
+
+    def create_state(self, index, weight):
+        import torch
+        w = weight.as_torch()
+        return tuple(torch.zeros_like(w, dtype=torch.float32) for _ in range(2))     # acc_g, acc_delta
+
+    def step(self, indices, weights, grads, states):     # adadelta.py:72-111
+        import torch
+        for index, weight, grad, state in zip(indices, weights, grads, states):
+            self._update_count(index)
+            lr = self._get_lr(index)
+            w, g = weight.as_torch(), grad.as_torch()
+            g = _prep_grad(self, index, w, g)
+            acc_g, acc_delta = state
+            acc_g.mul_(self.rho).add_((1. - self.rho) * torch.square(g))
+            delta = torch.sqrt(acc_delta + self.epsilon)
+            delta = delta / torch.sqrt(acc_g + self.epsilon) * g
+            acc_delta.mul_(self.rho).add_((1. - self.rho) * torch.square(delta))
+            w.sub_(lr * delta)
+
+
 class _LayerwiseAdaptive(Optimizer):
     """Shared part of LAMB / LANS / LARS: ``skip_nonfinite=True`` asks the store to leave weights and
     state alone when a merged gradient holds inf/nan (the AMP overflow skip, gluon/trainer.py:445-448,
@@ -743,8 +835,8 @@ class NativeUpdater(object):
     """Same call contract as :class:`Updater` (updater.py:39-93; ``index`` / ``grad`` / ``weight`` may be
     lists), but the whole list is updated IN PLACE by one fused launch (sequence) of the native engine
     -- what the reference does with ``multi_sgd_mom_update`` / ``multi_mp_sgd_*`` / ``multi_adamw`` /
-    ``multi_adabelief`` / ``rmsprop_update`` / ``signum_update`` / ``multi_lamb`` / ``multi_lans`` when parameters are
-    not updated on the kvstore (sgd.py:170-213, lamb.py:170-215).  One instance serves one device, like
+    ``multi_adabelief`` / ``rmsprop_update`` / ``signum_update`` / ``ftml_update`` / ``multi_lamb`` / ``multi_lans``, or
+    ``Adamax.step`` / ``AdaDelta.step`` (which have no operator), when parameters are not updated on the kvstore (sgd.py:170-213, lamb.py:170-215).  One instance serves one device, like
     ``Trainer._updaters[dev]``."""
 
     def __init__(self, optimizer):
