@@ -144,7 +144,7 @@ MXKV_DLL int MXKVStoreSendCommmandToServers(KVStoreHandle handle, int cmd_id, co
 /* Fused optimizer: what Python's Updater + sgd_update/adam_update ops do per key in the
  * reference (python/mxnet/optimizer/updater.py:39-93) happens inside the reduce kernel.
  * name: "sgd" | "nag" | "adam" | "adamw" | "adabelief" | "rmsprop" | "signum" | "ftml" | "adamax" | "adadelta" |
- * "test" | "lamb" | "lans" | "lars";
+ * "nadam" | "test" | "lamb" | "lans" | "lars";
  * kwargs use the reference's hyper-parameter names (learning_rate, wd, momentum, rescale_grad, clip_gradient, beta1,
  * beta2, epsilon, eta, multi_precision, lazy_update, correct_bias, lower_bound, upper_bound,
  * bias_correction, rho, centered, clip_weights, wd_lh).  rmsprop: centered=True selects rmspropalex_update; a
@@ -157,7 +157,11 @@ MXKV_DLL int MXKVStoreSendCommmandToServers(KVStoreHandle handle, int cmd_id, co
  * restated (the reference has no operator for either), every scalar parsed as a double and rounded once to float, as
  * Python hands it to an NDArray operation; class defaults learning_rate 0.002, beta1 0.9, beta2 0.999, epsilon 1e-8
  * (adamax) and learning_rate 1.0, rho 0.9, epsilon 1e-6 (adadelta); clip_gradient clips at 0 too, as step does, and
- * is off below 0 or None.  lamb / lans / lars
+ * is off below 0 or None.  nadam: Nadam.step restated the same way; class defaults learning_rate 0.001, beta1 0.9,
+ * beta2 0.999, epsilon 1e-8, schedule_decay 0.004; m_schedule sets the momentum-schedule product (without it,
+ * hyper-parameters re-sent to the current nadam keep the product, and a new one starts at 1), which every fused key
+ * update advances in call order (MXKVB200GetOptimizerScalar); clip as for adamax; calls are never deferred
+ * (MXKVB200SetDeferred), since reordering them would reorder the product.  lamb / lans / lars
  * additionally take skip_nonfinite=True: when any merged gradient of a push holds inf/nan, that push changes neither
  * weights nor optimizer state (the AMP overflow skip of gluon/trainer.py:445-448, decided on the device inside the
  * same launch sequence). */
@@ -172,8 +176,8 @@ MXKV_DLL int MXKVB200SetOptimizerMult(KVStoreHandle handle, int key, const char*
  * kvstore (multi_sgd_update / multi_sgd_mom_update / multi_mp_sgd_*, src/operator/optimizer_op-inl.h:
  * 207-375; nag_mom_update / mp_nag_mom_update per weight, :1029-1092; multi_adamw, multi_adabelief,
  * multi_lamb, multi_lans; rmsprop_update / rmspropalex_update per weight, :1905-2031; signsgd_update /
- * signum_update per weight, :2293-2379; ftml_update per weight, :1117-1206; Adamax.step / AdaDelta.step, which have
- * no operator).  Create the handle with MXKVStoreCreate("updater"), give it an optimizer with MXKVB200SetOptimizer, then every call updates all (weight, grad) pairs
+ * signum_update per weight, :2293-2379; ftml_update per weight, :1117-1206; Adamax.step / AdaDelta.step / Nadam.step,
+ * which have no operator; Nadam's schedule product advances once per pair, in pair order).  Create the handle with MXKVStoreCreate("updater"), give it an optimizer with MXKVB200SetOptimizer, then every call updates all (weight, grad) pairs
  * IN PLACE with one launch (sequence) on their GPU.  Optimizer state of an index is created on first
  * sight and is reachable through MXKVB200GetState / SetState / Get|SetUpdateCount.  One handle serves
  * one device, like the reference's `Trainer._updaters[dev]`.  Never collective.  grads == NULL only
@@ -187,7 +191,8 @@ MXKV_DLL int MXKVB200UpdaterStepEx(KVStoreHandle handle, uint32_t num, const cha
  * wd_mult; AdamW and AdaBelief: operator lr = 1 and eta = the bias-corrected learning rate; FTML: lr =
  * (1 - beta1^t) / (learning rate x lr_mult) and eta = 1 - beta2^t, the two powers of the update count t that
  * ftml_update takes per element, in float as the operator does; Adamax: lr = learning rate x lr_mult / (1 - beta1^t)
- * and eta = 1 - beta1; AdaDelta: eta = 1 - rho -- each computed in double and rounded once).  Host-only, no GPU
+ * and eta = 1 - beta1; AdaDelta: eta = 1 - rho; Nadam: eta = coef2 = 1 - beta2^t -- each computed in double and
+ * rounded once).  Host-only, no GPU
  * needed. */
 MXKV_DLL int MXKVB200GetKeyHyper(KVStoreHandle handle, int key, const char* str_key, float* lr, float* wd,
                                  float* eta);
@@ -205,8 +210,8 @@ MXKV_DLL int MXKVB200GetOverflow(KVStoreHandle handle, int* out);
 MXKV_DLL int MXKVB200MultiSumSq(uint32_t num, NDArrayHandle* arrays, float scale, NDArrayHandle out);
 MXKV_DLL int MXKVB200MultiAllFinite(uint32_t num, NDArrayHandle* arrays, int init_output, NDArrayHandle out);
 /* which: 0 stored value, 1 fp32 master weight, 2 state0 (momentum | mean | RMSProp var; centered RMSProp: mean;
- * Signum: the negated momentum, as the reference stores it; FTML: d; Adamax: mean; AdaDelta: acc_g),
- * 3 state1 (variance; FTML: v; Adamax: var, the max-norm; AdaDelta: acc_delta), 4 state2 (centered RMSProp momentum;
+ * Signum: the negated momentum, as the reference stores it; FTML: d; Adamax: mean; AdaDelta: acc_g; Nadam: mean),
+ * 3 state1 (variance; FTML: v; Adamax: var, the max-norm; AdaDelta: acc_delta; Nadam: var), 4 state2 (centered RMSProp momentum;
  * FTML: z).
  * Returns a NEW handle aliasing engine memory (free it with MXNDArrayFree); *out = NULL when the
  * state does not exist. */
@@ -216,6 +221,12 @@ MXKV_DLL int MXKVB200SetState(KVStoreHandle handle, int key, const char* str_key
                               NDArrayHandle value);
 MXKV_DLL int MXKVB200GetUpdateCount(KVStoreHandle handle, int key, const char* str_key, int64_t* out);
 MXKV_DLL int MXKVB200SetUpdateCount(KVStoreHandle handle, int key, const char* str_key, int64_t count);
+/* Store-wide scalars of the fused optimizer, as doubles.  name "m_schedule": Nadam's momentum-schedule product
+ * (Nadam.m_schedule, nadam.py:100), which every fused key update multiplies in call order -- the sorted keys of a
+ * push / pushpull, the pair order of MXKVB200UpdaterStep.  Set it to hand the product from one store to another
+ * (the per-device updaters of a Trainer share one optimizer object); host-only, no GPU needed. */
+MXKV_DLL int MXKVB200GetOptimizerScalar(KVStoreHandle handle, const char* name, double* out);
+MXKV_DLL int MXKVB200SetOptimizerScalar(KVStoreHandle handle, const char* name, double value);
 
 /* Wrap device/host memory owned by the embedding framework (no copy, no ownership). */
 MXKV_DLL int MXKVB200NDArrayFromPtr(void* data, const int64_t* shape, int ndim, int dev_type, int dev_id,

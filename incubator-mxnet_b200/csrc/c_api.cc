@@ -518,6 +518,20 @@ int MXKVB200SetUpdateCount(KVStoreHandle handle, int key, const char* str_key, i
   API_END();
 }
 
+int MXKVB200GetOptimizerScalar(KVStoreHandle handle, const char* name, double* out) {
+  API_BEGIN();
+  MXKV_CHECK(name != nullptr && out != nullptr) << "GetOptimizerScalar: null argument";
+  *out = KV(handle)->GetOptimizerScalar(name);
+  API_END();
+}
+
+int MXKVB200SetOptimizerScalar(KVStoreHandle handle, const char* name, double value) {
+  API_BEGIN();
+  MXKV_CHECK(name != nullptr) << "SetOptimizerScalar: null name";
+  KV(handle)->SetOptimizerScalar(name, value);
+  API_END();
+}
+
 int MXKVB200UpdaterStep(KVStoreHandle handle, uint32_t num, const int* keys, NDArrayHandle* weights,
                         NDArrayHandle* grads) {
   API_BEGIN();

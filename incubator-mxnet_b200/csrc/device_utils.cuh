@@ -293,8 +293,10 @@ __device__ __forceinline__ int find_work(const DenseLaunch& L, int64_t c, int* c
   return lo;
 }
 
-// the update's hyper-parameters for one entry: lr / wd / eta are per key, the rest per launch
-__device__ __forceinline__ Hyper make_hyper(const DenseLaunch& L, const TensorWork& tw, bool mp) {
+// the update's hyper-parameters for entry `idx`: lr / wd / eta are per key, the rest per launch.  Nadam's further
+// per-key scalars come from the launch's side array (DenseLaunch::nadam); no other kind reads it
+template <int OPT>
+__device__ __forceinline__ Hyper make_hyper(const DenseLaunch& L, const TensorWork& tw, bool mp, int idx) {
   Hyper h;
   h.lr = tw.lr; h.wd = tw.wd; h.eta = tw.eta;
   h.rescale = L.rescale; h.clip = L.clip; h.momentum = L.momentum;
@@ -302,6 +304,13 @@ __device__ __forceinline__ Hyper make_hyper(const DenseLaunch& L, const TensorWo
   h.rho = L.rho; h.clip_weights = L.clip_weights;
   h.wd_lh = L.wd_lh;
   h.mp = mp;
+  if constexpr (OPT == OPT_NADAM) {
+    const float4 s = L.nadam[idx];
+    h.c1 = L.one_minus_beta1; h.c2 = L.one_minus_beta2;
+    h.g_div = s.x; h.m_div = s.y; h.mom_t1 = s.z; h.c_mom_t = s.w;
+  } else {
+    (void)idx;
+  }
   return h;
 }
 

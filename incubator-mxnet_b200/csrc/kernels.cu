@@ -141,7 +141,7 @@ kv_dense_kernel(DenseLaunch L) {
   int cur = -1;
   for (int64_t c = blockIdx.x; c < L.total_chunks; c += gridDim.x) {
     const int lo = find_work(L, c, &cur, &tw);
-    const Hyper h = make_hyper(L, tw, sizeof(T) == 2 && L.mp_arith != 0);
+    const Hyper h = make_hyper<OPT>(L, tw, sizeof(T) == 2 && L.mp_arith != 0, lo);
 
     const int64_t cb = tw.begin + (c - L.chunk_prefix[lo]) * L.chunk_elems;
     const int64_t ce = (cb + L.chunk_elems < tw.end) ? cb + L.chunk_elems : tw.end;
@@ -330,7 +330,7 @@ kv_dense_bulk_kernel(DenseLaunch L) {
   for (int64_t i = 0; i < ntiles; ++i) {
     const int64_t c = tile_of(i);
     const int lo = find_work(L, c, &cur, &tw);
-    const Hyper h = make_hyper(L, tw, false);   // float32 keys only
+    const Hyper h = make_hyper<OPT>(L, tw, false, lo);   // float32 keys only
     const int64_t cb = tw.begin + (c - L.chunk_prefix[lo]) * tile;
     const int64_t ce = (cb + tile < tw.end) ? cb + tile : tw.end;
     const int nvec = static_cast<int>((ce - cb) >> 2);
@@ -531,7 +531,7 @@ kv_dense_nvls_kernel(DenseLaunch L) {
       __syncthreads();
       cur = k.lo;
     }
-    const Hyper h = make_hyper(L, tw, false);   // float32 keys only
+    const Hyper h = make_hyper<OPT>(L, tw, false, k.lo);   // float32 keys only
     const int64_t nvec = (k.ce - k.cb) >> 2;
     const int n_plain = tw.n_out - tw.n_mc;
     // state of all U packets first (independent HBM loads in flight together), then the arithmetic

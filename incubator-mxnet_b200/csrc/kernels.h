@@ -50,25 +50,27 @@ enum OptKind : int {
   OPT_FTML = 17,      // FTMLKernel                          optimizer_op-inl.h:1159-1177
   // no reference operator: the optimizer class's own `step`, one NDArray operation per rounding
   OPT_ADAMAX = 18,    // Adamax.step                         python/mxnet/optimizer/adamax.py:74-111
-  OPT_ADADELTA = 19   // AdaDelta.step                       python/mxnet/optimizer/adadelta.py:72-111
+  OPT_ADADELTA = 19,  // AdaDelta.step                       python/mxnet/optimizer/adadelta.py:72-111
+  OPT_NADAM = 20      // Nadam.step                          python/mxnet/optimizer/nadam.py:74-124
 };
-constexpr int kNumOptKinds = OPT_ADADELTA + 1;   // one past the last kind: the size of tables indexed by kind
+constexpr int kNumOptKinds = OPT_NADAM + 1;   // one past the last kind: the size of tables indexed by kind
 inline bool IsNormOpt(int kind) { return kind == OPT_LAMB || kind == OPT_LANS || kind == OPT_LARS; }
 
 // The fp32 state arrays an element-wise kind streams through update_one: s0 (momentum / mean / RMSProp var;
-// centered RMSProp: mean; Signum: the negated momentum; FTML: d; Adamax: mean; AdaDelta: acc_g), s1 (variance; FTML:
-// v; Adamax: the max-norm u; AdaDelta: acc_delta), s2 (centered RMSProp: momentum; FTML: z) -- the tuple order of the
+// centered RMSProp: mean; Signum: the negated momentum; FTML: d; Adamax: mean; AdaDelta: acc_g; Nadam: mean), s1
+// (variance; FTML: v; Adamax: the max-norm u; AdaDelta: acc_delta; Nadam: var), s2 (centered RMSProp: momentum; FTML: z) -- the tuple order of the
 // reference's create_state.  Every dense kernel loads and stores exactly
 // these, and the staged kernel counts them among its staged arrays.  The layer-wise adaptive kinds keep their state
 // rules with their launch sequence (KVStore::EnsureState).
 __host__ __device__ constexpr bool OptHasS0(int kind) {
   return kind == OPT_SGD_MOM || kind == OPT_ADAM || kind == OPT_ADAMW || kind == OPT_ADAM_STD || kind == OPT_NAG ||
          kind == OPT_ADABELIEF || kind == OPT_RMSPROP || kind == OPT_RMSPROP_CENTERED || kind == OPT_SIGNUM ||
-         kind == OPT_FTML || kind == OPT_ADAMAX || kind == OPT_ADADELTA;
+         kind == OPT_FTML || kind == OPT_ADAMAX || kind == OPT_ADADELTA || kind == OPT_NADAM;
 }
 __host__ __device__ constexpr bool OptHasS1(int kind) {
   return kind == OPT_ADAM || kind == OPT_ADAMW || kind == OPT_ADAM_STD || kind == OPT_ADABELIEF ||
-         kind == OPT_RMSPROP_CENTERED || kind == OPT_FTML || kind == OPT_ADAMAX || kind == OPT_ADADELTA;
+         kind == OPT_RMSPROP_CENTERED || kind == OPT_FTML || kind == OPT_ADAMAX || kind == OPT_ADADELTA ||
+         kind == OPT_NADAM;
 }
 __host__ __device__ constexpr bool OptHasS2(int kind) { return kind == OPT_RMSPROP_CENTERED || kind == OPT_FTML; }
 // The fp32 arrays a kind streams next to its gradients: the weight (every kind but OPT_NONE) and its state arrays.
@@ -97,7 +99,7 @@ struct OptKinds {
 };
 using ElementwiseOpts = OptKinds<OPT_SGD, OPT_SGD_MOM, OPT_ADAM, OPT_ADAMW, OPT_TEST, OPT_NAG, OPT_ADABELIEF,
                                  OPT_RMSPROP, OPT_RMSPROP_CENTERED, OPT_SIGNSGD, OPT_SIGNUM, OPT_FTML, OPT_ADAMAX,
-                                 OPT_ADADELTA>;
+                                 OPT_ADADELTA, OPT_NADAM>;
 
 enum SumOrder : int {
   ORDER_DEVICE = 0,  // ((in0+in1)+in2)+...                  ndarray_function-inl.h:457-486
@@ -124,7 +126,8 @@ struct alignas(16) TensorWork {
   float lr;          // per-key learning rate (lr_mult, scheduler, Adam / Adamax bias correction folded in; FTML:
                      //   (1-beta1^t)/lr)
   float wd;          // per-key weight decay
-  float eta;         // AdamW schedule multiplier (FTML: 1 - beta2^t; Adamax: 1 - beta1, AdaDelta: 1 - rho, in double)
+  float eta;         // AdamW schedule multiplier (FTML: 1 - beta2^t; Adamax: 1 - beta1, AdaDelta: 1 - rho, in double;
+                     //   Nadam: coef2 = 1 - beta2^t; its other per-key scalars: DenseLaunch::nadam)
   int n_src;
   int n_out;
   int flags;         // kWork* bits (WorkFlags)
@@ -207,6 +210,11 @@ struct DenseLaunch {
   float rho;                     // RMSProp: decay of the squared-gradient (and centered: gradient) averages
   float clip_weights;            // RMSProp: |new weight| <= clip_weights when >= 0 (< 0: off)
   float wd_lh;                   // Signum: decoupled weight decay, w *= 1 - lr*wd_lh before the sign step
+  // Nadam: four more per-key scalars than TensorWork has room for, one float4 per entry (nworks of them), uploaded
+  // with the work list right after the chunk prefix: (1 - m_schedule, 1 - m_schedule_next, momentum_t_1,
+  // 1 - momentum_t), each computed in double and rounded once (KVStore::NadamAdvance).  Null for every other kind.
+  const float4* nadam;
+  float one_minus_beta1, one_minus_beta2;   // Nadam: 1 - beta1 / 1 - beta2 computed in double, rounded once
 };
 
 // returns cudaError_t as int; never throws

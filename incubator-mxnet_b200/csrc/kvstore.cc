@@ -272,6 +272,9 @@ void KVStore::SetDeferred(bool on) {
 bool KVStore::Defer(int kind, const std::vector<int>& vkeys, const std::vector<int>& okeys,
                     const std::vector<NDArray>& vals, const std::vector<NDArray*>& outs, int priority) {
   if (!deferred_ || hier_ || updater_ != nullptr || gc_bits_ != 0) return false;
+  // Nadam's momentum schedule is one product over every key update in call order: reordering calls by priority
+  // would change it, so these calls are issued as they come
+  if (opt_.enabled && opt_.kind == OPT_NADAM) return false;
   for (auto& v : vals) if (!v.ctx().is_gpu() || v.stype() != kDefaultStorage) return false;
   for (NDArray* o : outs) if (!o->ctx().is_gpu() || o->stype() != kDefaultStorage) return false;
   for (int k : vkeys) { auto it = keys_.find(k); if (it == keys_.end() || it->second.stype != kDefaultStorage) return false; }
@@ -445,11 +448,15 @@ void KVStore::SetOptimizer(const std::string& name, const std::vector<std::pair<
     c.kind = OPT_ADAMAX; c.lr = 0.002; c.beta1 = 0.9; c.beta2 = 0.999; c.eps = static_cast<float>(1e-8);
   } else if (n == "adadelta") {
     c.kind = OPT_ADADELTA; c.lr = 1.0; c.rho_d = 0.9; c.rho = static_cast<float>(0.9); c.eps = static_cast<float>(1e-6);
+  } else if (n == "nadam") {      // nadam.py:58-67; clip as for Adamax
+    c.kind = OPT_NADAM; c.lr = 0.001; c.beta1 = 0.9; c.beta2 = 0.999; c.eps = static_cast<float>(1e-8);
+    c.schedule_decay = 0.004; c.m_schedule = 1.0;
   }
   else MXKV_FATAL() << "optimizer '" << name << "' has no fused kernel; register a Python updater instead";
-  // Adamax and AdaDelta restate their optimizer's Python `step`, where a scalar enters an NDArray operation as
+  // Adamax, AdaDelta and Nadam restate their optimizer's Python `step`, where a scalar enters an NDArray operation as
   // float32(double): parse as double, then round once (std::stof may round the decimal string differently)
-  const bool from_double = c.kind == OPT_ADAMAX || c.kind == OPT_ADADELTA;
+  const bool from_double = c.kind == OPT_ADAMAX || c.kind == OPT_ADADELTA || c.kind == OPT_NADAM;
+  bool have_m_schedule = false;
   auto to_float = [from_double](const std::string& v) {
     return from_double ? static_cast<float>(std::stod(v)) : std::stof(v);
   };
@@ -480,6 +487,8 @@ void KVStore::SetOptimizer(const std::string& name, const std::vector<std::pair<
     else if (k == "centered") centered = (v == "True" || v == "true" || v == "1");
     else if (k == "clip_weights") c.clip_weights = (v == "None" || v.empty()) ? -1.f : std::stof(v);
     else if (k == "wd_lh") c.wd_lh = std::stod(v);
+    else if (k == "schedule_decay") c.schedule_decay = std::stod(v);
+    else if (k == "m_schedule") { c.m_schedule = std::stod(v); have_m_schedule = true; }
     else MXKV_FATAL() << "unknown optimizer argument '" << k << "'";
   }
   if (c.kind == OPT_RMSPROP) {
@@ -502,6 +511,10 @@ void KVStore::SetOptimizer(const std::string& name, const std::vector<std::pair<
   if (c.kind == OPT_FTML && !(c.clip > 0.f)) c.clip = -1.f;
   if (c.kind == OPT_SGD && c.momentum != 0.f) c.kind = OPT_SGD_MOM;   // sgd.py:213-224
   if (c.kind == OPT_NAG && c.momentum == 0.f) c.kind = OPT_SGD;       // nag.py:59-63,141-154: no state, (mp_)sgd_update
+  // Nadam's schedule product: set by an explicit m_schedule; without one, hyper-parameters re-sent to the current
+  // Nadam (no reset_states) keep the product where the store's updates have taken it
+  if (c.kind == OPT_NADAM && !have_m_schedule && !reset_states && opt_.enabled && opt_.kind == OPT_NADAM)
+    c.m_schedule = opt_.m_schedule;
   MXKV_CHECK(!c.skip_nonfinite || IsNormOpt(c.kind)) << "skip_nonfinite is available for lamb / lans / lars";
   c.lr_mult = opt_.lr_mult;
   c.wd_mult = opt_.wd_mult;
@@ -598,6 +611,8 @@ bool KVStore::SkipsOnRescale() const {
 float KVStore::KeyEta(const KeyState& ks) const {
   if (EtaCarriesLR(opt_.kind)) return static_cast<float>(KeyLRd(ks) * opt_.eta_d);
   if (opt_.kind == OPT_FTML) return 1.0f - FtmlPow(opt_.beta2, ks.count);
+  // nadam.py:95: coef2 = 1. - self.beta2**t
+  if (opt_.kind == OPT_NADAM) return static_cast<float>(1. - std::pow(opt_.beta2, static_cast<double>(ks.count)));
   if (EtaIsComplement(opt_.kind)) return static_cast<float>(1.0 - (opt_.kind == OPT_ADAMAX ? opt_.beta1 : opt_.rho_d));
   return opt_.eta;
 }
@@ -618,6 +633,23 @@ double KVStore::KeyLRd(const KeyState& ks) const {
   // adamax.py:93: lr /= (1. - self.beta1**t)
   if (opt_.kind == OPT_ADAMAX) lr /= (1. - std::pow(opt_.beta1, static_cast<double>(ks.count)));
   return lr;
+}
+
+void KVStore::AdvanceCount(KeyState& ks) {
+  ks.count += 1;
+  if (opt_.kind == OPT_NADAM) NadamAdvance(ks);
+}
+
+// nadam.py:97-101, in double as Python computes it: the warming momentum schedule of update count t, and the
+// optimizer-wide product m_schedule, which this update multiplies.  The kernel's scalars are rounded once each.
+void KVStore::NadamAdvance(KeyState& ks) {
+  const double t = static_cast<double>(ks.count);
+  const double mom_t = opt_.beta1 * (1. - 0.5 * std::pow(0.96, t * opt_.schedule_decay));
+  const double mom_t1 = opt_.beta1 * (1. - 0.5 * std::pow(0.96, (t + 1.) * opt_.schedule_decay));
+  opt_.m_schedule = opt_.m_schedule * mom_t;
+  const double m_next = opt_.m_schedule * mom_t1;
+  ks.nadam = make_float4(static_cast<float>(1. - opt_.m_schedule), static_cast<float>(1. - m_next),
+                         static_cast<float>(mom_t1), static_cast<float>(1. - mom_t));
 }
 
 float KVStore::KeyWD(const KeyState& ks) const {
@@ -1174,7 +1206,7 @@ bool KVStore::HostPipelined(std::vector<Group>& groups, bool write_outs) {
       if (ks.has_state) GatherState(ks);
       EnsureState(ks, *r, mp);
       ks.state_world = 0;
-      ks.count += 1;
+      AdvanceCount(ks);
     }
     r = FindReplica(ks, dev);
     if (fused) SyncState(ks, *r);
@@ -1329,7 +1361,7 @@ void KVStore::ReduceUpdateCompressed(std::vector<Group>& groups, bool write_outs
     const int n_total = mp_mode ? world : n_src;
     const bool mp = fused && opt_.multi_precision;
     std::set<NDArray*> written;
-    if (fused) ks.count += 1;
+    if (fused) AdvanceCount(ks);
     const float lr = fused ? KeyLR(ks) : 0.f;
     const float wd = fused ? KeyWD(ks) : 0.f;
     for (int dev : consumers) {
@@ -1576,12 +1608,15 @@ bool KVStore::PlanEpochsMatch(const CallPlan& p) const {
 void KVStore::PlanPatch(CallPlan& p, bool commit_counts) {
   if (!p.fused) return;
   std::vector<std::array<float, 3>> hyper(p.keys.size());
+  const double m_schedule = opt_.m_schedule;
   for (size_t i = 0; i < p.keys.size(); ++i) {
     KeyState& ks = keys_.find(p.keys[i])->second;    // (not GetKey: a replay does not expire its own plan)
-    ks.count += 1;
+    const float4 nadam = ks.nadam;
+    AdvanceCount(ks);                                 // in the group order of the call, as a fresh build does
     hyper[i] = {KeyLR(ks), KeyWD(ks), KeyEta(ks)};
-    if (!commit_counts) ks.count -= 1;
+    if (!commit_counts) { ks.count -= 1; ks.nadam = nadam; }
   }
+  if (!commit_counts) opt_.m_schedule = m_schedule;
   for (auto& l : p.launches)
     for (size_t q = 0; q < l.per_part.size(); ++q)
       for (size_t e = 0; e < l.per_part[q].size(); ++e) {
@@ -2125,7 +2160,7 @@ void KVStore::KeyWorks(CallPlan& plan, const KeyBuild& k, const std::vector<std:
   const bool collective = plan.collective, two_shot = k.two_shot;
   float lr = 0.f, wd = 0.f;
   if (plan.fused) {
-    ks.count += 1;                 // Optimizer._update_count
+    AdvanceCount(ks);              // Optimizer._update_count
     lr = KeyLR(ks);
     wd = KeyWD(ks);
   }
@@ -2243,9 +2278,18 @@ void KVStore::LaunchWorks(const LaunchClassKey& ck, std::vector<std::vector<Tens
     prefix[w.size()] = acc;
     const int dev = part_dev[p];
     DeviceState& d = rt->Dev(dev);
+    // Nadam: the per-entry side array of the key scalars a TensorWork has no room for (DenseLaunch::nadam), in the
+    // same upload, 16-byte aligned after the chunk prefix
+    std::vector<float4> side;
+    if (opt_kind == OPT_NADAM) {
+      side.resize(w.size());
+      for (size_t i = 0; i < w.size(); ++i) side[i] = keys_.find(w[i].key)->second.nadam;
+    }
     const size_t wbytes = w.size() * sizeof(TensorWork);
     const size_t pbytes = prefix.size() * sizeof(int64_t);
-    const size_t bytes = wbytes + pbytes;
+    const size_t soff = wbytes + ((pbytes + 15) & ~static_cast<size_t>(15));
+    const size_t sbytes = side.size() * sizeof(float4);
+    const size_t bytes = side.empty() ? wbytes + pbytes : soff + sbytes;
     DeviceGuard dg(dev);
     // The upload is a copy on the engine stream between two kernels, a fixed cost of every launch: a list that is
     // byte-for-byte the resident one (the same keys pushed again with the same hyper-parameters) is read where it is.
@@ -2253,13 +2297,18 @@ void KVStore::LaunchWorks(const LaunchClassKey& ck, std::vector<std::vector<Tens
     const bool fits = bytes <= DeviceState::kResidentListBytes;
     const bool resident = fits && d.list_host.size() == bytes &&
                           std::memcmp(d.list_host.data(), w.data(), wbytes) == 0 &&
-                          std::memcmp(d.list_host.data() + wbytes, prefix.data(), pbytes) == 0;
+                          std::memcmp(d.list_host.data() + wbytes, prefix.data(), pbytes) == 0 &&
+                          (side.empty() || std::memcmp(d.list_host.data() + soff, side.data(), sbytes) == 0);
     size_t off = 0;
     char* list = d.list_dev;
     if (!resident) {
       off = d.ring.Alloc(bytes);
       std::memcpy(d.ring.host(off), w.data(), wbytes);
       std::memcpy(d.ring.host(off) + wbytes, prefix.data(), pbytes);
+      if (!side.empty()) {
+        std::memset(d.ring.host(off) + wbytes + pbytes, 0, soff - wbytes - pbytes);
+        std::memcpy(d.ring.host(off) + soff, side.data(), sbytes);
+      }
       if (!fits) list = d.ring.dev(off);
       CUDA_CALL(cudaMemcpyAsync(list, d.ring.host(off), bytes, cudaMemcpyHostToDevice, d.stream));
       if (fits) d.list_host.assign(d.ring.host(off), d.ring.host(off) + bytes);
@@ -2283,6 +2332,11 @@ void KVStore::LaunchWorks(const LaunchClassKey& ck, std::vector<std::vector<Tens
     L.beta1 = static_cast<float>(opt_.beta1); L.beta2 = static_cast<float>(opt_.beta2); L.eps = opt_.eps;
     L.rho = opt_.rho; L.clip_weights = opt_.clip_weights;
     L.wd_lh = static_cast<float>(opt_.wd_lh);
+    if (!side.empty()) {
+      L.nadam = reinterpret_cast<const float4*>(list + soff);
+      L.one_minus_beta1 = static_cast<float>(1. - opt_.beta1);
+      L.one_minus_beta2 = static_cast<float>(1. - opt_.beta2);
+    }
     L.sync.mode = ck.sync_mode;
     L.sync.world = n_part;
     L.sync.rank = p;
@@ -2599,6 +2653,17 @@ int64_t KVStore::GetUpdateCount(bool str_key, int ikey, const std::string& skey)
   LOCK();
   return GetKey(ResolveKey(str_key, ikey, skey)).count;
 }
+double KVStore::GetOptimizerScalar(const std::string& name) {
+  LOCK();
+  MXKV_CHECK(name == "m_schedule") << "unknown optimizer scalar '" << name << "'";
+  return opt_.m_schedule;
+}
+void KVStore::SetOptimizerScalar(const std::string& name, double value) {
+  LOCK();
+  MXKV_CHECK(name == "m_schedule") << "unknown optimizer scalar '" << name << "'";
+  opt_.m_schedule = value;
+}
+
 void KVStore::SetUpdateCount(bool str_key, int ikey, const std::string& skey, int64_t c) {
   LOCK_ONLY();
   const int key = ResolveKey(str_key, ikey, skey);

@@ -44,6 +44,9 @@ struct OptimizerConfig {
   float rho = 0.9f, clip_weights = -1.f;   // RMSProp (rmsprop.py:70-71); clip_weights < 0: off
   double rho_d = 0.9;         // rho as given (AdaDelta's 1 - rho is computed in double)
   double wd_lh = 0.0;         // Signum's decoupled weight decay (signum.py:67); double: signSGD adds it to wd in double
+  // Nadam (nadam.py:58-67): the schedule decay, and the optimizer's ONE momentum-schedule product, which every fused
+  // key update multiplies in call order (KVStore::NadamAdvance)
+  double schedule_decay = 0.004, m_schedule = 1.0;
   // LAMB / LANS / LARS (python/mxnet/optimizer/{lamb,lans,lars}.py)
   float lower_bound = -1.f, upper_bound = -1.f;   // bounds on the weight norm, < 0: not set
   bool bias_correction = true;                     // LAMB
@@ -96,6 +99,9 @@ struct KeyState {
   std::vector<int> shard_devs;   // devices (SP) / placeholder per rank (MP) of the shard owners
   std::vector<int> state_devs;   // the same for the optimizer-state shards (state_world entries)
   bool has_state = false;
+  // Nadam: the scalars of this key's latest update beyond lr / wd / eta (DenseLaunch::nadam), set when its count
+  // advances: 1 - m_schedule, 1 - m_schedule_next, momentum_t_1, 1 - momentum_t
+  float4 nadam{1.f, 1.f, 0.f, 0.f};
   // Bumped by every access through KVStore::GetKey, i.e. by every operation that may change this key's
   // replicas / layout / state flags; a cached launch plan (kvstore.h: CallPlan) is valid only while the
   // epochs of its keys are the ones it was recorded with.
@@ -181,6 +187,9 @@ class KVStore {
   int ResolveOverflow();
   void GetKeyHyper(bool str_key, int ikey, const std::string& skey, float* lr, float* wd, float* eta);
   int64_t GetUpdateCount(bool str_key, int ikey, const std::string& skey);
+  // store-wide scalars of the fused optimizer: "m_schedule" (Nadam's momentum-schedule product)
+  double GetOptimizerScalar(const std::string& name);
+  void SetOptimizerScalar(const std::string& name, double value);
   void SetUpdateCount(bool str_key, int ikey, const std::string& skey, int64_t c);
 
  private:
@@ -265,6 +274,9 @@ class KVStore {
   float KeyEta(const KeyState& ks) const;
   bool SkipsOnRescale() const;
   float KeyWD(const KeyState& ks) const;
+  // Optimizer._update_count for one fused key update; Nadam's schedule product advances with it, in call order
+  void AdvanceCount(KeyState& ks);
+  void NadamAdvance(KeyState& ks);
 
   // ---- multi-node ('dist_device_sync' over a configured Hierarchy, runtime.h) --------------------------
   // A push runs as: phase 1 = reduce(-scatter) of the node's values into this rank's staging slices; ONE

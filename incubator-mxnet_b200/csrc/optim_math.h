@@ -28,6 +28,9 @@ struct Hyper {
   bool mp;    // OPT_NAG only: MP_NAGMomKernel's grouping of the weight step (DenseLaunch::mp_arith)
   float rho, clip_weights;   // OPT_RMSPROP / OPT_RMSPROP_CENTERED (DenseLaunch::rho / clip_weights)
   float wd_lh;               // OPT_SIGNUM (DenseLaunch::wd_lh)
+  // OPT_NADAM only (make_hyper): 1 - beta1, 1 - beta2 per launch; per key 1 - m_schedule, 1 - m_schedule_next,
+  // momentum_t_1, 1 - momentum_t (DenseLaunch::nadam).  h.eta carries coef2 = 1 - beta2^t
+  float c1, c2, g_div, m_div, mom_t1, c_mom_t;
 };
 
 MXKV_HD float clipf(float x, float b) {   // mshadow_op::clip, mshadow_op.h:999-1009
@@ -167,6 +170,22 @@ MXKV_HD float update_one(float g, float w, float& s0, float& s1, const Hyper& h)
     const float ad = __fadd_rn(__fmul_rn(s1, h.rho), __fmul_rn(h.eta, __fmul_rn(cd, cd)));
     s0 = ag; s1 = ad;
     return __fsub_rn(w, __fmul_rn(h.lr, cd));
+  } else if (OPT == OPT_NADAM) {
+    // Nadam.step (s0 = mean, s1 = var), one NDArray operation per rounding, in step's order.  square(grad) and
+    // (1 - beta2) * square(grad) round separately.  The momentum schedule's scalars arrive per key, each computed in
+    // double and rounded once (KVStore::NadamAdvance): h.g_div = 1 - m_schedule, h.m_div = 1 - m_schedule_next,
+    // h.mom_t1 = momentum_t_1, h.c_mom_t = 1 - momentum_t, h.eta = coef2 = 1 - beta2^t
+    float r = __fmul_rn(g, h.rescale);
+    if (h.clip >= 0.0f) r = clipf(r, h.clip);
+    r = __fadd_rn(r, __fmul_rn(h.wd, w));
+    const float m = __fadd_rn(__fmul_rn(s0, h.beta1), __fmul_rn(h.c1, r));
+    const float v = __fadd_rn(__fmul_rn(s1, h.beta2), __fmul_rn(h.c2, __fmul_rn(r, r)));
+    s0 = m; s1 = v;
+    const float gp = __fdiv_rn(r, h.g_div);
+    const float mp = __fdiv_rn(m, h.m_div);
+    const float vp = __fdiv_rn(v, h.eta);
+    const float mb = __fadd_rn(__fmul_rn(h.mom_t1, mp), __fmul_rn(h.c_mom_t, gp));
+    return __fsub_rn(w, __fmul_rn(h.lr, __fdiv_rn(mb, __fadd_rn(__fsqrt_rn(vp), h.eps))));
   }
   return g;  // OPT_NONE
 }

@@ -102,15 +102,15 @@ kv_dense_tree_kernel(DenseLaunch L) {
   // of 512 threads resident (the residency the rendezvous grid is sized for)
   // (float32 keys of centered RMSProp and FTML, with three state arrays, take one element at a time for the same
   // reason; so do FTML's 16-bit keys, which spill 32 / 48 bytes at 64 registers with 4-element packets, and the
-  // float32 keys of Adamax and AdaDelta, which spill 12 / 16 bytes with them)
-  constexpr bool kOneElem = OPT == OPT_ADAMAX || OPT == OPT_ADADELTA;
+  // float32 keys of Adamax, AdaDelta and Nadam, which spill 12 / 16 / 16 bytes with them)
+  constexpr bool kOneElem = OPT == OPT_ADAMAX || OPT == OPT_ADADELTA || OPT == OPT_NADAM;
   constexpr int NV = (sizeof(T) == 2 && OPT == OPT_FTML) ? 1
                    : (sizeof(T) == 2 ? 4 : ((OptHasS2(OPT) || kOneElem) ? 1 : 16 / sizeof(T)));
   const bool native_half_add = (sizeof(T) == 2) && !L.fp32_accum && (OPT == OPT_NONE);
   int cur = -1;
   for (int64_t c = blockIdx.x; c < L.total_chunks; c += gridDim.x) {
     const int lo = find_work(L, c, &cur, &tw);
-    const Hyper h = make_hyper(L, tw, sizeof(T) == 2 && L.mp_arith != 0);
+    const Hyper h = make_hyper<OPT>(L, tw, sizeof(T) == 2 && L.mp_arith != 0, lo);
 
     const int64_t cb = tw.begin + (c - L.chunk_prefix[lo]) * L.chunk_elems;
     const int64_t ce = (cb + L.chunk_elems < tw.end) ? cb + L.chunk_elems : tw.end;

@@ -221,6 +221,7 @@ class KVStore(KVStoreBase):
         self._advance_counts(vkeys)
         fn = _LIB.MXKVStorePushEx if use_str else _LIB.MXKVStorePush
         check_call(fn(self.handle, n, ckeys, cvals, ctypes.c_int(priority)))
+        self._sync_scalars()
 
     def pull(self, key, out=None, priority=0, ignore_sparse=True):
         assert out is not None
@@ -234,6 +235,22 @@ class KVStore(KVStoreBase):
         self._advance_counts(vkeys)
         fn = _LIB.MXKVStorePushPullEx if use_str else _LIB.MXKVStorePushPull
         check_call(fn(self.handle, n, ckeys, m, cokeys, cvals, couts, ctypes.c_int(priority)))
+        self._sync_scalars()
+
+    def _sync_scalars(self):
+        """Nadam's ``m_schedule`` is one product for the whole optimizer, advanced by every fused key update in the
+        store: read back after each push, as the update counts are kept in step (``_advance_counts``), so that a
+        saved optimizer, a re-sent one and a Python ``step`` taking over all continue from it."""
+        if self._fused and getattr(self._optimizer, "fused_name", None) == "nadam":
+            self._optimizer.m_schedule = self._get_scalar("m_schedule")
+
+    def _get_scalar(self, name):
+        out = ctypes.c_double()
+        check_call(_LIB.MXKVB200GetOptimizerScalar(self.handle, c_str(name), ctypes.byref(out)))
+        return out.value
+
+    def _set_scalar(self, name, value):
+        check_call(_LIB.MXKVB200SetOptimizerScalar(self.handle, c_str(name), ctypes.c_double(value)))
 
     def broadcast(self, key, value, out, priority=0):
         vkeys, vals, use_str = _ctype_key_value(key, value)

@@ -1,10 +1,10 @@
 """Optimizer descriptors mirroring python/mxnet/optimizer/{optimizer,sgd,nag,adam,adamW,adabelief,rmsprop,signum,
-ftml,adamax,adadelta,updater}.py.
+ftml,adamax,adadelta,nadam,updater}.py.
 
 Two roles:
 * describe the hyper-parameters of the optimizers that have a fused kernel in the native
   engine (SGD / SGD-momentum / multi-precision SGD, NAG, Adam, AdamW, AdaBelief, RMSProp, Signum, FTML, Adamax,
-  AdaDelta, Test, and the layer-wise adaptive LAMB / LANS / LARS) -- ``KVStore.set_optimizer``
+  AdaDelta, Nadam, Test, and the layer-wise adaptive LAMB / LANS / LARS) -- ``KVStore.set_optimizer``
   hands them to ``MXKVB200SetOptimizer`` and the update then runs inside the reduce kernel;
 * provide the generic ``Updater`` callback (updater.py:39-93) for any other Optimizer object:
   the store reduces on the GPU and calls back into Python, exactly like the reference.  The
@@ -635,6 +635,65 @@ class AdaDelta(Optimizer):
             w.sub_(lr * delta)
 
 
+@register
+class Nadam(Optimizer):
+    """python/mxnet/optimizer/nadam.py: Adam with Nesterov momentum (Dozat, 2016).  The reference has no operator for
+    it: the fused kernel restates ``Nadam.step`` (nadam.py:74-124) one float32 operation per NDArray operation, every
+    Python scalar rounded once from its double::
+
+        grad = clip(grad * rescale_grad, clip_gradient) + wd * weight
+        momentum_t   = beta1 * (1 - 0.5 * 0.96**(t * schedule_decay))
+        momentum_t_1 = beta1 * (1 - 0.5 * 0.96**((t + 1) * schedule_decay))
+        m_schedule   = m_schedule * momentum_t            (ONE product for the optimizer, advanced by every update)
+        mean = beta1 * mean + (1 - beta1) * grad;  var = beta2 * var + (1 - beta2) * grad**2
+        mean_bar = momentum_t_1 * mean / (1 - m_schedule * momentum_t_1) + (1 - momentum_t) * grad / (1 - m_schedule)
+        weight = weight - lr * mean_bar / (sqrt(var / (1 - beta2**t)) + epsilon)
+
+    ``m_schedule`` is handed to the store with the other hyper-parameters and read back after every fused update, so
+    that it stands where the store's updates took it (a saved optimizer, a Python ``step`` taking over).
+    ``clip_gradient`` clips whenever it is not None, at 0 too; a negative one is off in the fused kernel."""
+    fused_name = "nadam"
+
+    def __init__(self, learning_rate=0.001, beta1=0.9, beta2=0.999, epsilon=1e-8, schedule_decay=0.004, **kwargs):
+        super(Nadam, self).__init__(learning_rate=learning_rate, **kwargs)
+        self.beta1, self.beta2, self.epsilon = beta1, beta2, epsilon
+        self.schedule_decay = schedule_decay
+        self.m_schedule = 1.
+
+    def fused_kwargs(self):
+        kw = super(Nadam, self).fused_kwargs()
+        kw.update(beta1=self.beta1, beta2=self.beta2, epsilon=self.epsilon, schedule_decay=self.schedule_decay,
+                  m_schedule=self.m_schedule)
+        return kw
+
+    def create_state(self, index, weight):
+        import torch
+        w = weight.as_torch()
+        return tuple(torch.zeros_like(w, dtype=torch.float32) for _ in range(2))     # mean, var
+
+    def step(self, indices, weights, grads, states):     # nadam.py:74-124
+        import torch
+        for index, weight, grad, state in zip(indices, weights, grads, states):
+            self._update_count(index)
+            lr = self._get_lr(index)
+            t = self._index_update_count[index]
+            w, g = weight.as_torch(), grad.as_torch()
+            g = _prep_grad(self, index, w, g)
+            coef2 = 1. - self.beta2 ** t
+            momentum_t = self.beta1 * (1. - 0.5 * (pow(0.96, t * self.schedule_decay)))
+            momentum_t_1 = self.beta1 * (1. - 0.5 * (pow(0.96, (t + 1) * self.schedule_decay)))
+            self.m_schedule = self.m_schedule * momentum_t
+            m_schedule_next = self.m_schedule * momentum_t_1
+            mean, var = state
+            mean.mul_(self.beta1).add_((1. - self.beta1) * g)
+            var.mul_(self.beta2).add_((1. - self.beta2) * torch.square(g))
+            grad_prime = g / (1. - self.m_schedule)
+            mean_prime = mean / (1. - m_schedule_next)
+            var_prime = var / coef2
+            mean_bar = momentum_t_1 * mean_prime + (1. - momentum_t) * grad_prime
+            w.sub_(lr * (mean_bar / (torch.sqrt(var_prime) + self.epsilon)))
+
+
 class _LayerwiseAdaptive(Optimizer):
     """Shared part of LAMB / LANS / LARS: ``skip_nonfinite=True`` asks the store to leave weights and
     state alone when a merged gradient holds inf/nan (the AMP overflow skip, gluon/trainer.py:445-448,
@@ -836,7 +895,7 @@ class NativeUpdater(object):
     lists), but the whole list is updated IN PLACE by one fused launch (sequence) of the native engine
     -- what the reference does with ``multi_sgd_mom_update`` / ``multi_mp_sgd_*`` / ``multi_adamw`` /
     ``multi_adabelief`` / ``rmsprop_update`` / ``signum_update`` / ``ftml_update`` / ``multi_lamb`` / ``multi_lans``, or
-    ``Adamax.step`` / ``AdaDelta.step`` (which have no operator), when parameters are not updated on the kvstore (sgd.py:170-213, lamb.py:170-215).  One instance serves one device, like
+    ``Adamax.step`` / ``AdaDelta.step`` / ``Nadam.step`` (which have no operator), when parameters are not updated on the kvstore (sgd.py:170-213, lamb.py:170-215).  One instance serves one device, like
     ``Trainer._updaters[dev]``."""
 
     def __init__(self, optimizer):
@@ -851,6 +910,7 @@ class NativeUpdater(object):
     def _sync(self):
         kw = self.optimizer.fused_kwargs()
         kw.pop("learning_rate", None)
+        kw.pop("m_schedule", None)    # (handed over around every call: __call__)
         if kw != self._kw:            # rescale_grad etc. changed (Trainer.step sets it per batch size)
             self._kv.set_optimizer(self.optimizer)
             self._kw = kw
@@ -888,8 +948,25 @@ class NativeUpdater(object):
             for i, c in before.items():
                 self._kv._set_count(i, c)
                 self._kv._synced.add(i)
+        # Nadam: the per-device updaters of a Trainer share one optimizer object and so one schedule product, which
+        # each call advances once per pair in pair order; it travels through the object between the devices' stores
+        nadam = self.optimizer.fused_name == "nadam"
+        if nadam:
+            if self.optimizer.aggregate_num > 1 and n > 1:
+                # updater.py:65-80: an aggregating updater groups the pairs by dtype (first seen first) before it steps
+                first = {}
+                for w in weight:
+                    first.setdefault(w.dtype, len(first))
+                order = sorted(range(n), key=lambda i: first[weight[i].dtype])
+                index, weight, grad = [index[i] for i in order], [weight[i] for i in order], [grad[i] for i in order]
+                wh = (ctypes.c_void_p * n)(*[w.handle.value for w in weight])
+                gh = (ctypes.c_void_p * n)(*[g.handle.value for g in grad])
+                keys = c_str_array(list(index)) if use_str else (ctypes.c_int * n)(*[int(i) for i in index])
+            self._kv._set_scalar("m_schedule", self.optimizer.m_schedule)
         check_call(fn(self._kv.handle, n, keys, wh, gh))
         self._kv._keys.update(index)
+        if nadam:
+            self.optimizer.m_schedule = self._kv._get_scalar("m_schedule")
 
     def get_states(self, dump_optimizer=False):
         return self._kv._dump_fused_states(dump_optimizer)

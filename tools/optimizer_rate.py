@@ -9,7 +9,9 @@ signSGD against the fused SGD (16 bytes each: read g, w; write stored w, out), a
 With `--pair ftml`: the fused FTML against the fused centered RMSProp (40 bytes per float32 element each: read g, w
 and three states; write stored w, three states, out), and FTML through the Python `step`.  With `--pair adamax` /
 `--pair adadelta`: the fused Adamax / AdaDelta against the fused Adam (32 bytes per float32 element each: read g, w,
-s0, s1; write stored w, s0, s1, out), and the optimizer through the Python `step`.
+s0, s1; write stored w, s0, s1, out), and the optimizer through the Python `step`.  With `--pair nadam`: the fused
+Nadam against the fused Adam (the same 32 bytes per element; Nadam's per-key schedule scalars ride along with the work
+list), and Nadam through the Python `step`.
 
 Two key sets: the bench sweep (9 float32 keys, 2^10 ... 2^26 elements) and ResNet-50's 193 gradient-carrying arrays
 (bench.py: keyset).  Both fused optimizers move the same bytes per element (read g, w, mom; write stored w, mom, out),
@@ -18,7 +20,7 @@ engine's stream (the Python path: host clock around a device synchronise, its to
 dense kernel variant that ran (launch counters), and one step checked against the CPU oracle.  The card's name and
 power limit are read with nvidia-smi in the same call and printed with the numbers.
 
-    python tools/optimizer_rate.py [--pair nag|adabelief|rmsprop|signum|ftml|adamax|adadelta] [--steps 200] [--warmup 20] [--rounds 3]
+    python tools/optimizer_rate.py [--pair nag|adabelief|rmsprop|signum|ftml|adamax|adadelta|nadam] [--steps 200] [--warmup 20] [--rounds 3]
 """
 import argparse
 import ctypes
@@ -40,18 +42,20 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 KW = dict(learning_rate=0.01, momentum=0.9, wd=1e-4)
 KW_ADAPTIVE = dict(learning_rate=0.001, wd=1e-4)
 KW_FTML = dict(learning_rate=0.0025, wd=1e-4)
-KW_STEP = {"adamax": dict(learning_rate=0.002, wd=1e-4), "adadelta": dict(learning_rate=1.0, wd=1e-4)}
+KW_STEP = {"adamax": dict(learning_rate=0.002, wd=1e-4), "adadelta": dict(learning_rate=1.0, wd=1e-4),
+           "nadam": dict(learning_rate=0.001, wd=1e-4)}
 # --pair: (baseline, optimizer under test) pairs, alternated in one process; the python step is timed for the first
-# optimizer under test where it was the only way to run it (NAG, RMSProp, Signum, FTML, Adamax, AdaDelta)
+# optimizer under test where it was the only way to run it (NAG, RMSProp, Signum, FTML, Adamax, AdaDelta, Nadam)
 PAIRS = {"nag": [("sgd", "nag")], "adabelief": [("adam", "adabelief")],
          "rmsprop": [("sgd", "rmsprop"), ("adam", "rmsprop_centered")],
          "signum": [("sgd", "signum"), ("sgd_plain", "signsgd")],
-         "ftml": [("rmsprop_centered", "ftml")], "adamax": [("adam", "adamax")], "adadelta": [("adam", "adadelta")]}
-PYTHON_STEP = ("nag", "rmsprop", "signum", "ftml", "adamax", "adadelta")
+         "ftml": [("rmsprop_centered", "ftml")], "adamax": [("adam", "adamax")], "adadelta": [("adam", "adadelta")],
+         "nadam": [("adam", "nadam")]}
+PYTHON_STEP = ("nag", "rmsprop", "signum", "ftml", "adamax", "adadelta", "nadam")
 LABELS = {"sgd": "sgd_momentum", "nag": "nag", "adam": "adam", "adabelief": "adabelief", "rmsprop": "rmsprop",
           "rmsprop_centered": "rmsprop (centered)", "sgd_plain": "sgd", "signum": "signum",
           "signsgd": "signum (momentum 0: signsgd)", "ftml": "ftml",
-          "adamax": "adamax", "adadelta": "adadelta"}
+          "adamax": "adamax", "adadelta": "adadelta", "nadam": "nadam"}
 VARIANTS = ("per_thread", "bulk", "nvls", "tree")
 
 
@@ -91,7 +95,7 @@ class Case(object):
                "adabelief": mx.optimizer.AdaBelief, "rmsprop": mx.optimizer.RMSProp,
                "rmsprop_centered": mx.optimizer.RMSProp, "sgd_plain": mx.optimizer.SGD, "signum": mx.optimizer.Signum,
                "signsgd": mx.optimizer.Signum, "ftml": mx.optimizer.FTML,
-               "adamax": mx.optimizer.Adamax, "adadelta": mx.optimizer.AdaDelta}[optname]
+               "adamax": mx.optimizer.Adamax, "adadelta": mx.optimizer.AdaDelta, "nadam": mx.optimizer.Nadam}[optname]
         opt = cls(**dict(self.kw, **({} if fused else {"use_fused_step": False})))
         self.kv.set_optimizer(opt)
         self.grads = [mx.nd.array(g, mx.gpu(0)) for g in self.grads_np]
@@ -129,6 +133,9 @@ class Case(object):
         elif self.optname == "adadelta":
             import adadelta_oracle as AD
             oopt = AD.OracleAdaDelta(**self.kw)
+        elif self.optname == "nadam":
+            import nadam_oracle as NA
+            oopt = NA.OracleNadam(**self.kw)
         else:
             oopt = O.OracleOptimizer("sgd" if self.optname == "sgd_plain" else self.optname, **self.kw)
         exact, close = True, True
