@@ -212,7 +212,7 @@ struct DenseLaunch {
   float wd_lh;                   // Signum: decoupled weight decay, w *= 1 - lr*wd_lh before the sign step
   // Nadam: four more per-key scalars than TensorWork has room for, one float4 per entry (nworks of them), uploaded
   // with the work list right after the chunk prefix: (1 - m_schedule, 1 - m_schedule_next, momentum_t_1,
-  // 1 - momentum_t), each computed in double and rounded once (KVStore::NadamAdvance).  Null for every other kind.
+  // 1 - momentum_t), each computed in double and rounded once (KVStore::KeyScalars).  Null for every other kind.
   const float4* nadam;
   float one_minus_beta1, one_minus_beta2;   // Nadam: 1 - beta1 / 1 - beta2 computed in double, rounded once
 };

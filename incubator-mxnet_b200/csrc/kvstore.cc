@@ -589,15 +589,9 @@ static float FtmlPow(double beta, int64_t count) {
   return static_cast<float>(std::pow(static_cast<double>(static_cast<float>(beta)), static_cast<double>(t)));
 }
 
-// Adamax and AdaDelta: the complement that `step` writes as `(1. - beta1) * grad` / `(1. - rho) * square(...)` --
-// computed in double, then rounded once.  1.f - float(beta1) is a different number for most betas (0.1f against
-// 0.100000024f at beta1 = 0.9)
-static bool EtaIsComplement(int kind) { return kind == OPT_ADAMAX || kind == OPT_ADADELTA; }
-
-float KVStore::KeyLR(const KeyState& ks) const {
-  if (EtaCarriesLR(opt_.kind)) return 1.0f;
-  if (opt_.kind == OPT_FTML) return (1.0f - FtmlPow(opt_.beta1, ks.count)) / static_cast<float>(KeyLRd(ks));
-  return static_cast<float>(KeyLRd(ks));
+// nadam.py:97-98, in double as Python computes it: the warming momentum schedule of update count t
+static double NadamMomentum(const OptimizerConfig& o, double t) {
+  return o.beta1 * (1. - 0.5 * std::pow(0.96, t * o.schedule_decay));
 }
 
 // `_adamw_update`, `_adabelief_update` and their multi / mp forms leave everything untouched when the
@@ -608,16 +602,8 @@ bool KVStore::SkipsOnRescale() const {
          (!std::isfinite(opt_.rescale) || opt_.rescale == 0.f);
 }
 
-float KVStore::KeyEta(const KeyState& ks) const {
-  if (EtaCarriesLR(opt_.kind)) return static_cast<float>(KeyLRd(ks) * opt_.eta_d);
-  if (opt_.kind == OPT_FTML) return 1.0f - FtmlPow(opt_.beta2, ks.count);
-  // nadam.py:95: coef2 = 1. - self.beta2**t
-  if (opt_.kind == OPT_NADAM) return static_cast<float>(1. - std::pow(opt_.beta2, static_cast<double>(ks.count)));
-  if (EtaIsComplement(opt_.kind)) return static_cast<float>(1.0 - (opt_.kind == OPT_ADAMAX ? opt_.beta1 : opt_.rho_d));
-  return opt_.eta;
-}
-
-double KVStore::KeyLRd(const KeyState& ks) const {
+KeyStep KVStore::KeyScalars(const KeyState& ks) const {
+  KeyStep s;
   // Optimizer._get_lr (optimizer.py) then, for Adam, the host-side bias correction of
   // adam.py:166-175 -- all in double like Python, rounded to float once.
   double lr = opt_.lr;
@@ -632,33 +618,48 @@ double KVStore::KeyLRd(const KeyState& ks) const {
   }
   // adamax.py:93: lr /= (1. - self.beta1**t)
   if (opt_.kind == OPT_ADAMAX) lr /= (1. - std::pow(opt_.beta1, static_cast<double>(ks.count)));
-  return lr;
-}
-
-void KVStore::AdvanceCount(KeyState& ks) {
-  ks.count += 1;
-  if (opt_.kind == OPT_NADAM) NadamAdvance(ks);
-}
-
-// nadam.py:97-101, in double as Python computes it: the warming momentum schedule of update count t, and the
-// optimizer-wide product m_schedule, which this update multiplies.  The kernel's scalars are rounded once each.
-void KVStore::NadamAdvance(KeyState& ks) {
-  const double t = static_cast<double>(ks.count);
-  const double mom_t = opt_.beta1 * (1. - 0.5 * std::pow(0.96, t * opt_.schedule_decay));
-  const double mom_t1 = opt_.beta1 * (1. - 0.5 * std::pow(0.96, (t + 1.) * opt_.schedule_decay));
-  opt_.m_schedule = opt_.m_schedule * mom_t;
-  const double m_next = opt_.m_schedule * mom_t1;
-  ks.nadam = make_float4(static_cast<float>(1. - opt_.m_schedule), static_cast<float>(1. - m_next),
-                         static_cast<float>(mom_t1), static_cast<float>(1. - mom_t));
-}
-
-float KVStore::KeyWD(const KeyState& ks) const {
+  s.lr_d = lr;
   double wd = opt_.wd;
-  auto it = opt_.wd_mult.find(ks.key);
+  it = opt_.wd_mult.find(ks.key);
   if (it != opt_.wd_mult.end()) wd *= it->second;
   // signsgd_update is handed wd + wd_lh, summed in Python (double) and not multiplied by wd_mult (signum.py:156-158)
   if (opt_.kind == OPT_SIGNSGD) wd += opt_.wd_lh;
-  return static_cast<float>(wd);
+  s.wd = static_cast<float>(wd);
+  s.lr = static_cast<float>(s.lr_d);
+  s.eta = opt_.eta;
+  if (EtaCarriesLR(opt_.kind)) {
+    s.lr = 1.0f;
+    s.eta = static_cast<float>(s.lr_d * opt_.eta_d);
+  } else if (opt_.kind == OPT_FTML) {
+    s.lr = (1.0f - FtmlPow(opt_.beta1, ks.count)) / static_cast<float>(s.lr_d);
+    s.eta = 1.0f - FtmlPow(opt_.beta2, ks.count);
+  } else if (opt_.kind == OPT_ADAMAX || opt_.kind == OPT_ADADELTA) {
+    // the complement that `step` writes as `(1. - beta1) * grad` / `(1. - rho) * square(...)` -- computed in double,
+    // then rounded once.  1.f - float(beta1) is a different number for most betas (0.1f against 0.100000024f at 0.9)
+    s.eta = static_cast<float>(1.0 - (opt_.kind == OPT_ADAMAX ? opt_.beta1 : opt_.rho_d));
+  } else if (opt_.kind == OPT_NADAM) {
+    // nadam.py:95-101: coef2 = 1. - self.beta2**t, and the schedule at t and t + 1 with the optimizer-wide product
+    // m_schedule that this update has multiplied (StepKey); in double as Python computes them, each rounded once
+    const double t = static_cast<double>(ks.count);
+    s.eta = static_cast<float>(1. - std::pow(opt_.beta2, t));
+    const double mom_t = NadamMomentum(opt_, t), mom_t1 = NadamMomentum(opt_, t + 1.);
+    const double m_next = opt_.m_schedule * mom_t1;
+    s.nadam = make_float4(static_cast<float>(1. - opt_.m_schedule), static_cast<float>(1. - m_next),
+                          static_cast<float>(mom_t1), static_cast<float>(1. - mom_t));
+  }
+  if (IsNormOpt(opt_.kind)) {
+    // bias correction denominators: power::Map(beta, step) in float (multi_lamb.cc:64-69)
+    const float tcount = static_cast<float>(ks.count);
+    s.c1 = 1.0f - std::pow(static_cast<float>(opt_.beta1), tcount);
+    s.c2 = 1.0f - std::pow(static_cast<float>(opt_.beta2), tcount);
+  }
+  return s;
+}
+
+void KVStore::StepKey(KeyState& ks) {
+  ks.count += 1;
+  if (opt_.kind == OPT_NADAM) opt_.m_schedule = opt_.m_schedule * NadamMomentum(opt_, static_cast<double>(ks.count));
+  ks.step = KeyScalars(ks);
 }
 
 // ---------------------------------------------------------------------------
@@ -916,7 +917,7 @@ void KVStore::PushImpl(const std::vector<int>& keys, const std::vector<NDArray>&
       PushRowSparse(GetKey(uniq[i]), grouped[i]);
       continue;
     }
-    if (SkipsOnRescale()) { ks.count += 1; continue; }
+    if (SkipsOnRescale()) { StepKey(ks); continue; }
     // BASELINE configs[0], the reference's CPU-runnable case: ONE host-resident value pushed to a key that has
     // never met a GPU, nothing to run on it (no updater, no optimizer, no compression).  The reference does no
     // arithmetic here either -- Reduce hands a single value back as it is (comm.h:128-131) and the store copies it
@@ -1021,7 +1022,7 @@ void KVStore::PushPullImpl(const std::vector<int>& vkeys, const std::vector<int>
     return;
   }
   if (SkipsOnRescale()) {
-    for (int key : vu) PeekKey(key).count += 1;
+    for (int key : vu) StepKey(PeekKey(key));
     PullImpl(okeys, outs, priority, true);
     return;
   }
@@ -1206,7 +1207,7 @@ bool KVStore::HostPipelined(std::vector<Group>& groups, bool write_outs) {
       if (ks.has_state) GatherState(ks);
       EnsureState(ks, *r, mp);
       ks.state_world = 0;
-      AdvanceCount(ks);
+      StepKey(ks);
     }
     r = FindReplica(ks, dev);
     if (fused) SyncState(ks, *r);
@@ -1214,8 +1215,6 @@ bool KVStore::HostPipelined(std::vector<Group>& groups, bool write_outs) {
       o.fresh = (&o == r);
       if (fused && &o != r) o.state_fresh = false;
     }
-    const float lr = fused ? KeyLR(ks) : 0.f;
-    const float wd = fused ? KeyWD(ks) : 0.f;
     const int n_src = static_cast<int>(g.vals.size());
     const size_t slot_stride = ((static_cast<size_t>(std::min<int64_t>(seg_elems, ks.size)) * esize + 255) / 256) * 256;
     for (int64_t b = 0; b < ks.size || (ks.size == 0 && b == 0); b += seg_elems) {
@@ -1234,7 +1233,7 @@ bool KVStore::HostPipelined(std::vector<Group>& groups, bool write_outs) {
       CUDA_CALL(cudaEventRecord(d.ev_h2d[slot], d.copy_in));
       // stage 2: fused reduce(+update) on the element range [b, e)
       CUDA_CALL(cudaStreamWaitEvent(d.stream, d.ev_h2d[slot], 0));
-      TensorWork tw = ReplicaWork(ks, *r, mp, b, e, lr, wd);
+      TensorWork tw = ReplicaWork(ks, *r, fused, mp, b, e);
       if (coll) {               // rank q's slot as mapped here; the start rendezvous orders it after q's H2D
         tw.n_src = world;
         for (int q = 0; q < world; ++q)
@@ -1361,9 +1360,7 @@ void KVStore::ReduceUpdateCompressed(std::vector<Group>& groups, bool write_outs
     const int n_total = mp_mode ? world : n_src;
     const bool mp = fused && opt_.multi_precision;
     std::set<NDArray*> written;
-    if (fused) AdvanceCount(ks);
-    const float lr = fused ? KeyLR(ks) : 0.f;
-    const float wd = fused ? KeyWD(ks) : 0.f;
+    if (fused) StepKey(ks);
     for (int dev : consumers) {
       touch(dev);
       EnsureReplica(ks, dev);
@@ -1375,7 +1372,7 @@ void KVStore::ReduceUpdateCompressed(std::vector<Group>& groups, bool write_outs
       float* deq = nullptr;
       CUDA_CALL(cudaMallocAsync(reinterpret_cast<void**>(&deq), static_cast<size_t>(n_total) * std::max<int64_t>(ks.size, 4) * 4, s));
       temps.push_back({deq, dev});
-      TensorWork tw = ReplicaWork(ks, r, mp, 0, ks.size, lr, wd);
+      TensorWork tw = ReplicaWork(ks, r, fused, mp, 0, ks.size);
       tw.n_src = n_total;
       for (int k = 0; k < n_total; ++k) {
         const uint32_t* codes;
@@ -1607,22 +1604,22 @@ bool KVStore::PlanEpochsMatch(const CallPlan& p) const {
 // the only per-call data of a repeated call: update counts and the per-key scalars derived from them
 void KVStore::PlanPatch(CallPlan& p, bool commit_counts) {
   if (!p.fused) return;
-  std::vector<std::array<float, 3>> hyper(p.keys.size());
+  std::vector<KeyStep> steps(p.keys.size());
   const double m_schedule = opt_.m_schedule;
   for (size_t i = 0; i < p.keys.size(); ++i) {
     KeyState& ks = keys_.find(p.keys[i])->second;    // (not GetKey: a replay does not expire its own plan)
-    const float4 nadam = ks.nadam;
-    AdvanceCount(ks);                                 // in the group order of the call, as a fresh build does
-    hyper[i] = {KeyLR(ks), KeyWD(ks), KeyEta(ks)};
-    if (!commit_counts) { ks.count -= 1; ks.nadam = nadam; }
+    const KeyStep prev = ks.step;
+    StepKey(ks);                                      // in the group order of the call, as a fresh build does
+    steps[i] = ks.step;
+    if (!commit_counts) { ks.count -= 1; ks.step = prev; }
   }
   if (!commit_counts) opt_.m_schedule = m_schedule;
   for (auto& l : p.launches)
     for (size_t q = 0; q < l.per_part.size(); ++q)
       for (size_t e = 0; e < l.per_part[q].size(); ++e) {
         TensorWork& tw = l.per_part[q][e];
-        const auto& h = hyper[l.key_idx[q][e]];
-        tw.lr = h[0]; tw.wd = h[1]; tw.eta = h[2];
+        const KeyStep& st = steps[l.key_idx[q][e]];
+        tw.lr = st.lr; tw.wd = st.wd; tw.eta = st.eta;
       }
 }
 
@@ -2158,12 +2155,7 @@ void KVStore::KeyWorks(CallPlan& plan, const KeyBuild& k, const std::vector<std:
   KeyState& ks = k.ks;
   const int n_part = static_cast<int>(plan.part_dev.size());
   const bool collective = plan.collective, two_shot = k.two_shot;
-  float lr = 0.f, wd = 0.f;
-  if (plan.fused) {
-    AdvanceCount(ks);              // Optimizer._update_count
-    lr = KeyLR(ks);
-    wd = KeyWD(ks);
-  }
+  if (plan.fused) StepKey(ks);     // Optimizer._update_count
   LaunchClassKey ck{collective ? SYNC_WRITE_PEERS : SYNC_NONE, ks.dtype, k.mp ? 1 : 0};
   ck.nvls = k.nvls ? 1 : 0;
   ck.tree = k.tree != nullptr ? 1 : 0;
@@ -2176,9 +2168,9 @@ void KVStore::KeyWorks(CallPlan& plan, const KeyBuild& k, const std::vector<std:
   const int64_t shard = two_shot ? ShardLen(ks.size, n_part) : ks.size;
   l.busiest.push_back(std::min<int64_t>(ks.size, shard));
   for (int p = k.first; p <= k.last; ++p) {
-    TensorWork tw = two_shot ? ReplicaWork(ks, *k.rep[p], k.mp, std::min<int64_t>(ks.size, shard * p),
-                                           std::min<int64_t>(ks.size, shard * (p + 1)), lr, wd)
-                             : ReplicaWork(ks, *k.rep[p], k.mp, 0, ks.size, lr, wd);
+    TensorWork tw = two_shot ? ReplicaWork(ks, *k.rep[p], plan.fused, k.mp, std::min<int64_t>(ks.size, shard * p),
+                                           std::min<int64_t>(ks.size, shard * (p + 1)))
+                             : ReplicaWork(ks, *k.rep[p], plan.fused, k.mp, 0, ks.size);
     if (k.nvls) {                  // the switch sums the replicas: one multicast "source"
       tw.n_src = 1;
       tw.src[0] = k.g().vals[0].mc_data();
@@ -2283,7 +2275,7 @@ void KVStore::LaunchWorks(const LaunchClassKey& ck, std::vector<std::vector<Tens
     std::vector<float4> side;
     if (opt_kind == OPT_NADAM) {
       side.resize(w.size());
-      for (size_t i = 0; i < w.size(); ++i) side[i] = keys_.find(w[i].key)->second.nadam;
+      for (size_t i = 0; i < w.size(); ++i) side[i] = keys_.find(w[i].key)->second.step.nadam;
     }
     const size_t wbytes = w.size() * sizeof(TensorWork);
     const size_t pbytes = prefix.size() * sizeof(int64_t);
@@ -2368,8 +2360,8 @@ void KVStore::LaunchWorks(const LaunchClassKey& ck, std::vector<std::vector<Tens
   }
 }
 
-TensorWork KVStore::ReplicaWork(const KeyState& ks, const Replica& r, bool mp, int64_t begin, int64_t end, float lr,
-                                float wd) const {
+TensorWork KVStore::ReplicaWork(const KeyState& ks, const Replica& r, bool fused, bool mp, int64_t begin,
+                                int64_t end) const {
   TensorWork tw;
   std::memset(&tw, 0, sizeof(tw));
   tw.w = r.local.data();
@@ -2378,7 +2370,8 @@ TensorWork KVStore::ReplicaWork(const KeyState& ks, const Replica& r, bool mp, i
   tw.s1 = r.s1.is_none() ? nullptr : static_cast<float*>(r.s1.data());
   tw.s2 = r.s2.is_none() ? nullptr : static_cast<float*>(r.s2.data());
   tw.begin = begin; tw.end = end;
-  tw.lr = lr; tw.wd = wd; tw.eta = KeyEta(ks); tw.key = ks.key;
+  if (fused) { tw.lr = ks.step.lr; tw.wd = ks.step.wd; tw.eta = ks.step.eta; }
+  tw.key = ks.key;
   return tw;
 }
 
@@ -2597,7 +2590,7 @@ void KVStore::UpdaterStep(bool str_keys, const std::vector<int>& ikeys, const st
     r->fresh = true;
     ks.local_world = 0;
     if (bind_only) continue;
-    if (SkipsOnRescale()) { ks.count += 1; continue; }
+    if (SkipsOnRescale()) { StepKey(ks); continue; }
     if (grads[i].stype() == kRowSparseStorage) { sparse.emplace_back(key, grads[i]); continue; }
     Group grp;
     grp.key = key;
@@ -2644,9 +2637,10 @@ void KVStore::GetKeyHyper(bool str_key, int ikey, const std::string& skey, float
   LOCK();
   MXKV_CHECK(opt_.enabled) << "no fused optimizer is set";
   const KeyState& ks = GetKey(ResolveKey(str_key, ikey, skey));
-  if (lr) *lr = KeyLR(ks);
-  if (wd) *wd = KeyWD(ks);
-  if (eta) *eta = KeyEta(ks);
+  const KeyStep s = KeyScalars(ks);
+  if (lr) *lr = s.lr;
+  if (wd) *wd = s.wd;
+  if (eta) *eta = s.eta;
 }
 
 int64_t KVStore::GetUpdateCount(bool str_key, int ikey, const std::string& skey) {

@@ -45,7 +45,7 @@ struct OptimizerConfig {
   double rho_d = 0.9;         // rho as given (AdaDelta's 1 - rho is computed in double)
   double wd_lh = 0.0;         // Signum's decoupled weight decay (signum.py:67); double: signSGD adds it to wd in double
   // Nadam (nadam.py:58-67): the schedule decay, and the optimizer's ONE momentum-schedule product, which every fused
-  // key update multiplies in call order (KVStore::NadamAdvance)
+  // key update multiplies in call order (KVStore::StepKey)
   double schedule_decay = 0.004, m_schedule = 1.0;
   // LAMB / LANS / LARS (python/mxnet/optimizer/{lamb,lans,lars}.py)
   float lower_bound = -1.f, upper_bound = -1.f;   // bounds on the weight norm, < 0: not set
@@ -85,6 +85,15 @@ typedef NDArray Replica::*ReplicaArray;
 inline constexpr ReplicaArray kReplicaState[] = {&Replica::w32, &Replica::s0, &Replica::s1, &Replica::s2};
 constexpr int kNumReplicaState = static_cast<int>(sizeof(kReplicaState) / sizeof(kReplicaState[0]));
 
+// Every scalar one fused update of a key hands its kernels (KVStore::KeyScalars): TensorWork's lr / wd / eta,
+// NormWork's lr_d and bias corrections c1 / c2, and Nadam's DenseLaunch::nadam entry (1 - m_schedule,
+// 1 - m_schedule_next, momentum_t_1, 1 - momentum_t).
+struct KeyStep {
+  float lr = 0.f, wd = 0.f, eta = 0.f, c1 = 0.f, c2 = 0.f;
+  double lr_d = 0.0;
+  float4 nadam{1.f, 1.f, 0.f, 0.f};
+};
+
 struct KeyState {
   int key = 0;
   std::vector<int64_t> shape;
@@ -99,9 +108,7 @@ struct KeyState {
   std::vector<int> shard_devs;   // devices (SP) / placeholder per rank (MP) of the shard owners
   std::vector<int> state_devs;   // the same for the optimizer-state shards (state_world entries)
   bool has_state = false;
-  // Nadam: the scalars of this key's latest update beyond lr / wd / eta (DenseLaunch::nadam), set when its count
-  // advances: 1 - m_schedule, 1 - m_schedule_next, momentum_t_1, 1 - momentum_t
-  float4 nadam{1.f, 1.f, 0.f, 0.f};
+  KeyStep step;                  // the scalars of this key's latest fused update, set when its count advances
   // Bumped by every access through KVStore::GetKey, i.e. by every operation that may change this key's
   // replicas / layout / state flags; a cached launch plan (kvstore.h: CallPlan) is valid only while the
   // epochs of its keys are the ones it was recorded with.
@@ -225,9 +232,10 @@ class KVStore {
   std::vector<Dest> KeyDests(CallPlan& p, KeyBuild& k);
   void KeyWorks(CallPlan& p, const KeyBuild& k, const std::vector<std::vector<const void*>>& srcptr,
                 const std::vector<Dest>& dests);
-  // an entry that updates replica r of ks over [begin, end) (weight, fp32 master, optimizer state, key scalars);
-  // sources, destinations and flags are the caller's
-  TensorWork ReplicaWork(const KeyState& ks, const Replica& r, bool mp, int64_t begin, int64_t end, float lr, float wd) const;
+  // an entry that updates replica r of ks over [begin, end) (weight, fp32 master, optimizer state; a fused call's
+  // ks.step scalars, else zeros, which no OPT_NONE kernel reads and which keep unfused lists byte-equal); sources,
+  // destinations and flags are the caller's
+  TensorWork ReplicaWork(const KeyState& ks, const Replica& r, bool fused, bool mp, int64_t begin, int64_t end) const;
   // busiest[i]: number of elements the busiest rank processes for entry i (fixes the common grid)
   void LaunchWorks(const LaunchClassKey& ck, std::vector<std::vector<TensorWork>>& per_part,
                    const std::vector<int64_t>& busiest, int opt_kind, const std::vector<int>& part_dev);
@@ -253,9 +261,9 @@ class KVStore {
   void RowSparseKeyFor(KeyState& ks);
   bool RowSparseFused() const;
   RspSources PublishRowSparse(const KeyState& ks, Replica& r, const NDArray& v, bool fill);
-  RspRowArgs RowArgs(const KeyState& ks, const Replica& r, const RspSources& S, bool merge, bool update, bool assign,
-                     float lr, float wd) const;
-  void MergeRows(KeyState& ks, Replica& r, const RspSources& S, int64_t cap, bool update, bool assign, float lr, float wd);
+  RspRowArgs RowArgs(const KeyState& ks, const Replica& r, const RspSources& S, bool merge, bool update,
+                     bool assign) const;
+  void MergeRows(KeyState& ks, Replica& r, const RspSources& S, int64_t cap, bool update, bool assign);
   void InitRowSparseKey(KeyState& ks, const NDArray& v);
   void PullDenseFromRowSparse(KeyState& ks, const std::vector<NDArray*>& outs);
   void BroadcastFromRank0(KeyState& ks, Replica& r);
@@ -269,14 +277,12 @@ class KVStore {
   void SyncState(KeyState& ks, Replica& r);
   void GatherState(KeyState& ks);
   int DefaultDevice();
-  double KeyLRd(const KeyState& ks) const;
-  float KeyLR(const KeyState& ks) const;
-  float KeyEta(const KeyState& ks) const;
   bool SkipsOnRescale() const;
-  float KeyWD(const KeyState& ks) const;
-  // Optimizer._update_count for one fused key update; Nadam's schedule product advances with it, in call order
-  void AdvanceCount(KeyState& ks);
-  void NadamAdvance(KeyState& ks);
+  // every scalar of a fused update of ks at its current count (and Nadam's current schedule product)
+  KeyStep KeyScalars(const KeyState& ks) const;
+  // the one place a fused update is counted (Optimizer._update_count, in call order; Nadam's schedule product
+  // advances with it), run or skipped: derives the update's scalars into ks.step
+  void StepKey(KeyState& ks);
 
   // ---- multi-node ('dist_device_sync' over a configured Hierarchy, runtime.h) --------------------------
   // A push runs as: phase 1 = reduce(-scatter) of the node's values into this rank's staging slices; ONE

@@ -5,7 +5,6 @@
 // only on facts all ranks share, so paired blocks meet at every rendezvous.
 #include "kvstore.h"
 #include "norm_kernels.h"
-#include <cmath>
 #include <cstring>
 #include <functional>
 #include <map>
@@ -93,12 +92,9 @@ void KVStore::LaunchNormWorks(std::vector<NormClass>& classes, int opt_kind, con
         n.psum = part.psum + prefix[i] * kPsumStride;
         n.nrm = static_cast<float*>(r->nrm.data());
         n.begin = t.begin; n.end = t.end;
-        n.lr_d = KeyLRd(ks);
+        n.lr_d = ks.step.lr_d;
         n.lr = t.lr; n.wd = t.wd;
-        // bias correction denominators: power::Map(beta, step) in float (multi_lamb.cc:64-69)
-        const float tcount = static_cast<float>(ks.count);
-        n.c1 = 1.0f - std::pow(static_cast<float>(opt_.beta1), tcount);
-        n.c2 = 1.0f - std::pow(static_cast<float>(opt_.beta2), tcount);
+        n.c1 = ks.step.c1; n.c2 = ks.step.c2;
         n.n_src = t.n_src; n.n_out = t.n_out;
         n.flags = (t.flags & kWorkVec16) | (opt_.no_trust.count(ks.key) ? 2 : 0);
         // a sharded (two-shot) key: every rank holds the sums of its shard only

@@ -211,7 +211,7 @@ RspSources KVStore::PublishRowSparse(const KeyState& ks, Replica& r, const NDArr
 // the summed rows) goes to r's merge workspace.  `update`: the store's optimizer with r's state -- lazily on the touched
 // rows (lazy_update), else afterwards over the whole table (MergeRows).  `assign`: the merged rows replace the table.
 RspRowArgs KVStore::RowArgs(const KeyState& ks, const Replica& r, const RspSources& S, bool merge, bool update,
-                            bool assign, float lr, float wd) const {
+                            bool assign) const {
   const bool lazy = update && opt_.lazy_update;
   RspRowArgs A;
   std::memset(&A, 0, sizeof(A));
@@ -224,9 +224,10 @@ RspRowArgs KVStore::RowArgs(const KeyState& ks, const Replica& r, const RspSourc
   A.row_len = ks.size / ks.shape[0];
   A.opt = lazy ? opt_.kind : OPT_NONE;
   A.assign = assign ? 1 : 0;
-  A.lr = lr; A.wd = wd; A.rescale = opt_.rescale; A.clip = opt_.clip; A.momentum = opt_.momentum;
+  A.rescale = opt_.rescale; A.clip = opt_.clip; A.momentum = opt_.momentum;
   A.beta1 = static_cast<float>(opt_.beta1); A.beta2 = static_cast<float>(opt_.beta2); A.eps = opt_.eps;
   if (update) {
+    A.lr = ks.step.lr; A.wd = ks.step.wd;
     A.s0 = r.s0.is_none() ? nullptr : static_cast<float*>(r.s0.data());
     A.s1 = r.s1.is_none() ? nullptr : static_cast<float*>(r.s1.data());
   }
@@ -239,12 +240,11 @@ RspRowArgs KVStore::RowArgs(const KeyState& ks, const Replica& r, const RspSourc
 
 // The union + gather-sum kernels over sources S (up to `cap` rows each) on replica r, into its merge workspace, with
 // RowArgs' update / assignment; an update without lazy_update then runs the reference's standard update.
-void KVStore::MergeRows(KeyState& ks, Replica& r, const RspSources& S, int64_t cap, bool update, bool assign, float lr,
-                        float wd) {
+void KVStore::MergeRows(KeyState& ks, Replica& r, const RspSources& S, int64_t cap, bool update, bool assign) {
   Runtime* rt = Runtime::Get();
   cudaStream_t s = rt->Dev(r.dev).stream;
   EnsureRspWorkspace(ks, r, S.n, cap);
-  const RspRowArgs A = RowArgs(ks, r, S, true, update, assign, lr, wd);
+  const RspRowArgs A = RowArgs(ks, r, S, true, update, assign);
   // push without updater: local = merged (kvstore_local.h:279-284) -- rows outside the union vanish
   if (assign) CUDA_CALL(cudaMemsetAsync(r.local.data(), 0, r.local.nbytes(), s));
   CheckLaunch(LaunchRspSum(S, A, static_cast<int32_t*>(r.rsp_first.data()), static_cast<int32_t*>(r.rsp_pf.data()),
@@ -259,7 +259,7 @@ void KVStore::MergeRows(KeyState& ks, Replica& r, const RspSources& S, int64_t c
     CUDA_CALL(cudaMemsetAsync(gd, 0, static_cast<size_t>(ks.size) * 4, s));
     CheckLaunch(LaunchRspScatter(gd, r.rsp_merged.idx_ptr(), r.rsp_merged.d_nnz(), r.rsp_merged.cap_rows(), A.row_len,
                                  static_cast<const float*>(r.rsp_merged.data()), s), "rsp_scatter");
-    TensorWork tw = ReplicaWork(ks, r, false, 0, ks.size, lr, wd);
+    TensorWork tw = ReplicaWork(ks, r, true, false, 0, ks.size);
     tw.src[0] = gd; tw.n_src = 1;
     tw.out[0] = r.local.data(); tw.n_out = 1;
     tw.flags = ks.size % 4 == 0 ? WorkFlags(tw, false) : 0;   // (tables of other sizes keep the scalar path)
@@ -324,9 +324,7 @@ void KVStore::PushRowSparse(KeyState& ks, const std::vector<NDArray>& vals) {
       if (std::find(work_devs.begin(), work_devs.end(), r.dev) == work_devs.end()) r.state_fresh = false;
   }
 
-  if (fused) ks.count += 1;
-  const float lr = fused ? KeyLR(ks) : 0.f;
-  const float wd = fused ? KeyWD(ks) : 0.f;
+  if (fused) StepKey(ks);
 
   // ---- MP: publish this rank's gradient in the symmetric staging area ---------------------------
   const int world = mp_mode ? pg->world() : 1;
@@ -349,7 +347,7 @@ void KVStore::PushRowSparse(KeyState& ks, const std::vector<NDArray>& vals) {
       for (int k = 0; k < n_src; ++k) SourceOn(S, k, vals[k], L, dev, temps);
     }
     if (fused_path) {
-      RspRowArgs A = RowArgs(ks, r, S, false, true, false, lr, wd);    // (no union is materialised)
+      RspRowArgs A = RowArgs(ks, r, S, false, true, false);    // (no union is materialised)
       RspStage St;
       std::memset(&St, 0, sizeof(St));
       const SyncArgs sync = world > 1 ? GroupSync(SYNC_WRITE_PEERS) : LocalSync(dev);
@@ -397,7 +395,7 @@ void KVStore::PushRowSparse(KeyState& ks, const std::vector<NDArray>& vals) {
       CheckLaunch(LaunchRspPushFused(dev, S, A, St, sync, est_rows, s), "rsp_push_fused");
       for (void* t : tmp_src) if (t) CUDA_CALL(cudaFreeAsync(t, s));
     } else {
-      MergeRows(ks, r, S, cap, fused, !fused && !callback, lr, wd);
+      MergeRows(ks, r, S, cap, fused, !fused && !callback);
     }
     for (void* t : temps) CUDA_CALL(cudaFreeAsync(t, s));
     r.fresh = true;
@@ -449,9 +447,7 @@ void KVStore::HierPushRowSparse(KeyState& ks, const std::vector<NDArray>& vals) 
   MXKV_CHECK(!v.ctx().is_gpu() || v.ctx().dev_id == dev) << "value must live on GPU " << dev << " or on the host";
   PublishNnz(v);
   Replica& r = EnsureReplica(ks, dev);
-  if (fused) { EnsureState(ks, r, false); SyncState(ks, r); ks.count += 1; }
-  const float lr = fused ? KeyLR(ks) : 0.f;
-  const float wd = fused ? KeyWD(ks) : 0.f;
+  if (fused) { EnsureState(ks, r, false); SyncState(ks, r); StepKey(ks); }
   std::vector<void*> temps;
 
   // ---- (1) the node's merge ---------------------------------------------------------------------------------
@@ -465,7 +461,7 @@ void KVStore::HierPushRowSparse(KeyState& ks, const std::vector<NDArray>& vals) 
     S.n = 1;
     SourceOn(S, 0, v, L, dev, temps);
   }
-  MergeRows(ks, r, S, cap, false, false, lr, wd);
+  MergeRows(ks, r, S, cap, false, false);
 
   // ---- (2) gather the nodes' merged gradients ------------------------------------------------------------------
   int64_t* cnt = nullptr;                  // [nodes] row counts, device
@@ -505,7 +501,7 @@ void KVStore::HierPushRowSparse(KeyState& ks, const std::vector<NDArray>& vals) 
     S2.val[q] = val_all + static_cast<size_t>(q) * cap2 * L;
     S2.nnz[q] = cnt + q;
   }
-  MergeRows(ks, r, S2, cap2, fused, !fused, lr, wd);
+  MergeRows(ks, r, S2, cap2, fused, !fused);
   for (void* t : temps) CUDA_CALL(cudaFreeAsync(t, s));
   r.fresh = true;
   ks.local_world = 0;

@@ -135,7 +135,7 @@ MXKV_HD float update_one(float g, float w, float& s0, float& s1, const Hyper& h)
     return h.clip_weights >= 0.0f ? clipf(wn, h.clip_weights) : wn;
   } else if (OPT == OPT_SIGNSGD) {
     // SignSGDKernel: the sign of the summed gradient as it arrives -- rescale_grad and clip_gradient do not enter;
-    // wd is wd + wd_lh (KVStore::KeyWD).  lr * sign is exact.
+    // wd is wd + wd_lh (KVStore::KeyScalars).  lr * sign is exact.
     return __fsub_rn(__fmul_rn(__fsub_rn(1.f, __fmul_rn(h.lr, h.wd)), w), __fmul_rn(h.lr, signf(g)));
   } else if (OPT == OPT_SIGNUM) {
     // SignumKernel (s0 = mom, the NEGATED average: the weight step is + lr * sign(mom))
@@ -147,9 +147,9 @@ MXKV_HD float update_one(float g, float w, float& s0, float& s1, const Hyper& h)
     s0 = m;
     return __fadd_rn(__fmul_rn(__fsub_rn(1.f, __fmul_rn(h.lr, h.wd_lh)), w), __fmul_rn(h.lr, signf(m)));
   } else if (OPT == OPT_ADAMAX) {
-    // Adamax.step (s0 = mean, s1 = var, the max-norm u), one NDArray operation per rounding.  Per key (KVStore::KeyLR /
-    // KeyEta): h.lr = lr / (1 - beta1^t) and h.eta = 1 - beta1, each computed in double and rounded once, as Python
-    // hands a scalar to an NDArray operation
+    // Adamax.step (s0 = mean, s1 = var, the max-norm u), one NDArray operation per rounding.  Per key
+    // (KVStore::KeyScalars): h.lr = lr / (1 - beta1^t) and h.eta = 1 - beta1, each computed in double and rounded once,
+    // as Python hands a scalar to an NDArray operation
     float r = __fmul_rn(g, h.rescale);
     if (h.clip >= 0.0f) r = clipf(r, h.clip);
     r = __fadd_rn(r, __fmul_rn(h.wd, w));
@@ -159,7 +159,7 @@ MXKV_HD float update_one(float g, float w, float& s0, float& s1, const Hyper& h)
     return __fsub_rn(w, __fmul_rn(h.lr, __fdiv_rn(m, __fadd_rn(u, h.eps))));
   } else if (OPT == OPT_ADADELTA) {
     // AdaDelta.step (s0 = acc_g, s1 = acc_delta), one NDArray operation per rounding; h.eta = 1 - rho computed in
-    // double and rounded once (KVStore::KeyEta).  The step size is taken from the OLD acc_delta
+    // double and rounded once (KVStore::KeyScalars).  The step size is taken from the OLD acc_delta
     float r = __fmul_rn(g, h.rescale);
     if (h.clip >= 0.0f) r = clipf(r, h.clip);
     r = __fadd_rn(r, __fmul_rn(h.wd, w));
@@ -173,7 +173,7 @@ MXKV_HD float update_one(float g, float w, float& s0, float& s1, const Hyper& h)
   } else if (OPT == OPT_NADAM) {
     // Nadam.step (s0 = mean, s1 = var), one NDArray operation per rounding, in step's order.  square(grad) and
     // (1 - beta2) * square(grad) round separately.  The momentum schedule's scalars arrive per key, each computed in
-    // double and rounded once (KVStore::NadamAdvance): h.g_div = 1 - m_schedule, h.m_div = 1 - m_schedule_next,
+    // double and rounded once (KVStore::KeyScalars): h.g_div = 1 - m_schedule, h.m_div = 1 - m_schedule_next,
     // h.mom_t1 = momentum_t_1, h.c_mom_t = 1 - momentum_t, h.eta = coef2 = 1 - beta2^t
     float r = __fmul_rn(g, h.rescale);
     if (h.clip >= 0.0f) r = clipf(r, h.clip);
@@ -209,7 +209,7 @@ MXKV_HD float update_one(float g, float w, float& s0, float& s1, float& s2, cons
     const float wn = __fadd_rn(w, d);
     return h.clip_weights >= 0.0f ? clipf(wn, h.clip_weights) : wn;
   } else if constexpr (OPT == OPT_FTML) {
-    // FTMLKernel (s0 = d, s1 = v, s2 = z).  The two powers of t arrive per key (KVStore::KeyLR / KeyEta):
+    // FTMLKernel (s0 = d, s1 = v, s2 = z).  The two powers of t arrive per key (KVStore::KeyScalars):
     // h.lr = (1 - beta1^t) / lr and h.eta = 1 - beta2^t, so that
     //   v = beta2*v + (1-beta2)*r*r;  d_t = h.lr * (sqrt(v / h.eta) + eps)
     //   z = (beta1*z + (1-beta1)*r) - (d_t - beta1*d)*w;  d = d_t;  w = -z / d_t

@@ -2,7 +2,7 @@
 on float32 numpy arrays.  The reference has no operator for AdaDelta (its ``use_fused_step`` defaults to False and
 there is no ``fused_step``), so ``step`` itself is the definition.
 
-* ``adadelta_scalars``        -- the per-key scalars the engine hands the kernel (KVStore::KeyLR / KeyEta):
+* ``adadelta_scalars``        -- the per-key scalars the engine hands the kernel (KVStore::KeyScalars):
   ``lr_op = float32(lr)`` with ``lr`` the double learning rate x lr_mult, and ``eta_op = float32(1 - rho)``, the
   complement ``step`` writes as ``(1. - self.rho) * square(...)``, computed in double and rounded once.
 

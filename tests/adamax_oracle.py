@@ -2,10 +2,10 @@
 float32 numpy arrays, and the optimizer bookkeeping that drives it.  The reference has no operator for Adamax (its
 ``use_fused_step`` defaults to False and there is no ``fused_step``), so ``step`` itself is the definition.
 
-* ``adamax_scalars``          -- the two per-key scalars the engine hands the kernel for update count t (KVStore::KeyLR /
-  KeyEta): ``lr_op = float32(lr / (1 - beta1**t))`` with ``lr`` the double learning rate x lr_mult (adamax.py:91-93),
-  and ``eta_op = float32(1 - beta1)``, the complement ``step`` writes as ``(1. - self.beta1) * grad`` -- both computed
-  in double and rounded once.
+* ``adamax_scalars``          -- the two per-key scalars the engine hands the kernel for update count t
+  (KVStore::KeyScalars): ``lr_op = float32(lr / (1 - beta1**t))`` with ``lr`` the double learning rate x lr_mult
+  (adamax.py:91-93), and ``eta_op = float32(1 - beta1)``, the complement ``step`` writes as ``(1. - self.beta1) *
+  grad`` -- both computed in double and rounded once.
 
 * ``adamax_update``           -- adamax.py:95-111, states ``mean``, ``var`` (the max-norm u)::
 

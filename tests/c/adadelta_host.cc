@@ -6,7 +6,7 @@
 
 using namespace mxkv;
 
-// s0 = acc_g, s1 = acc_delta; lr_op = lr and eta_op = 1 - rho, the per-key scalars of KVStore::KeyLR / KeyEta
+// s0 = acc_g, s1 = acc_delta; lr_op = lr and eta_op = 1 - rho, the per-key scalars of KVStore::KeyScalars
 extern "C" int host_adadelta(int64_t n, const float* g, float* w, float* s0, float* s1, float lr_op, float wd,
                              float eta_op, float rho, float eps, float rescale, float clip) {
   Hyper h;

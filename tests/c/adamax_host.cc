@@ -6,8 +6,8 @@
 
 using namespace mxkv;
 
-// s0 = mean, s1 = var; lr_op = lr / (1 - beta1^t) and eta_op = 1 - beta1, the per-key scalars of KVStore::KeyLR /
-// KeyEta
+// s0 = mean, s1 = var; lr_op = lr / (1 - beta1^t) and eta_op = 1 - beta1, the per-key scalars of
+// KVStore::KeyScalars
 extern "C" int host_adamax(int64_t n, const float* g, float* w, float* s0, float* s1, float lr_op, float wd,
                            float eta_op, float beta1, float beta2, float eps, float rescale, float clip) {
   Hyper h;

@@ -6,8 +6,8 @@
 
 using namespace mxkv;
 
-// s0 = d, s1 = v, s2 = z; lr_op = (1 - beta1^t) / lr and eta_op = 1 - beta2^t, the per-key scalars of KVStore::KeyLR /
-// KeyEta
+// s0 = d, s1 = v, s2 = z; lr_op = (1 - beta1^t) / lr and eta_op = 1 - beta2^t, the per-key scalars of
+// KVStore::KeyScalars
 extern "C" int host_ftml(int64_t n, const float* g, float* w, float* s0, float* s1, float* s2, float lr_op, float wd,
                          float eta_op, float beta1, float beta2, float eps, float rescale, float clip) {
   Hyper h;

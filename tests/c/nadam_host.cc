@@ -7,7 +7,7 @@
 using namespace mxkv;
 
 // s0 = mean, s1 = var.  Per launch c1 = 1 - beta1, c2 = 1 - beta2; per key lr, coef2 (the entry's eta) and the side
-// array's 1 - m_schedule, 1 - m_schedule_next, momentum_t_1, 1 - momentum_t (KVStore::NadamAdvance)
+// array's 1 - m_schedule, 1 - m_schedule_next, momentum_t_1, 1 - momentum_t (KVStore::KeyScalars)
 extern "C" int host_nadam(int64_t n, const float* g, float* w, float* s0, float* s1, float lr, float wd, float coef2,
                           float g_div, float m_div, float mom_t1, float c_mom_t, float beta1, float beta2, float c1,
                           float c2, float eps, float rescale, float clip) {

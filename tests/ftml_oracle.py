@@ -1,9 +1,9 @@
 """FTML for the CPU oracle (test infrastructure): the reference's fused kernel restated operation by operation on float32
 numpy arrays, and the optimizer bookkeeping that drives it.
 
-* ``ftml_scalars``            -- the two per-key scalars the engine hands the kernel for update count t (KVStore::KeyLR /
-  KeyEta): ``t`` cast to float as the operator casts it, ``p = float(pow(float(beta), t))`` computed in double and
-  rounded once, then ``lr_op = (1 - p1) / lr`` and ``eta_op = 1 - p2`` in float -- the operator's
+* ``ftml_scalars``            -- the two per-key scalars the engine hands the kernel for update count t
+  (KVStore::KeyScalars): ``t`` cast to float as the operator casts it, ``p = float(pow(float(beta), t))`` computed
+  in double and rounded once, then ``lr_op = (1 - p1) / lr`` and ``eta_op = 1 - p2`` in float -- the operator's
   ``(1 - pow(beta1, t)) / lr`` and ``1 - pow(beta2, t)``, evaluated once per key.
 
 * ``ftml_update``             -- FTMLKernel (src/operator/optimizer_op-inl.h:1159-1177), states ``d``, ``v``, ``z``::

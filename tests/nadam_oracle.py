@@ -4,8 +4,7 @@ float32 numpy arrays, and the optimizer bookkeeping that drives it.  The referen
 
 * ``nadam_scalars``           -- nadam.py:95-101 in double for update count t and the optimizer's momentum-schedule
   product ``m_schedule`` as it stands before this update: returns the advanced product (a double, the caller's state)
-  and the per-key scalars the engine hands the kernel, each rounded once to float32 (KVStore::KeyEta /
-  KVStore::NadamAdvance)::
+  and the per-key scalars the engine hands the kernel, each rounded once to float32 (KVStore::KeyScalars)::
 
       coef2 = 1 - beta2**t
       momentum_t   = beta1 * (1 - 0.5 * 0.96**(t * schedule_decay))
