@@ -602,6 +602,17 @@ bool KVStore::SkipsOnRescale() const {
          (!std::isfinite(opt_.rescale) || opt_.rescale == 0.f);
 }
 
+// The reference reduces every push before its updater runs (kvstore_local.h:240-280), so under compression a
+// skipped step still quantises each pushed value against its residual (comm.h:556-605); only the operator then
+// leaves weight and state alone.  Without compression there is nothing to reduce for: the step is only counted.
+void KVStore::SkipStep(std::vector<Group>& groups) {
+  if (gc_bits_ != 0) {
+    ReduceUpdateCompressed(groups, false, true);
+    return;
+  }
+  for (auto& g : groups) StepKey(PeekKey(g.key));
+}
+
 KeyStep KVStore::KeyScalars(const KeyState& ks) const {
   KeyStep s;
   // Optimizer._get_lr (optimizer.py) then, for Adam, the host-side bias correction of
@@ -910,14 +921,20 @@ void KVStore::PushImpl(const std::vector<int>& keys, const std::vector<NDArray>&
         << "Unexpected storage type detected during kvstore push: " << nd.stype();
     return true;
   });
-  std::vector<Group> dense;
+  std::vector<Group> dense, skipped;
   for (size_t i = 0; i < uniq.size(); ++i) {
     KeyState& ks = PeekKey(uniq[i]);
     if (grouped[i][0].stype() == kRowSparseStorage || ks.stype == kRowSparseStorage) {
       PushRowSparse(GetKey(uniq[i]), grouped[i]);
       continue;
     }
-    if (SkipsOnRescale()) { StepKey(ks); continue; }
+    if (SkipsOnRescale()) {
+      Group g;
+      g.key = uniq[i];
+      g.vals = grouped[i];
+      skipped.push_back(g);
+      continue;
+    }
     // BASELINE configs[0], the reference's CPU-runnable case: ONE host-resident value pushed to a key that has
     // never met a GPU, nothing to run on it (no updater, no optimizer, no compression).  The reference does no
     // arithmetic here either -- Reduce hands a single value back as it is (comm.h:128-131) and the store copies it
@@ -940,6 +957,7 @@ void KVStore::PushImpl(const std::vector<int>& keys, const std::vector<NDArray>&
     g.vals = grouped[i];
     dense.push_back(g);
   }
+  if (!skipped.empty()) SkipStep(skipped);
   raw_single_ = dense.size() == uniq.size();        // the whole call as ONE reduce: a launch plan may be recorded
   if (!dense.empty()) ReduceUpdate(dense, false);
   raw_single_ = false;
@@ -1021,16 +1039,16 @@ void KVStore::PushPullImpl(const std::vector<int>& vkeys, const std::vector<int>
     PullImpl(okeys, outs, priority, true);
     return;
   }
-  if (SkipsOnRescale()) {
-    for (int key : vu) StepKey(PeekKey(key));
-    PullImpl(okeys, outs, priority, true);
-    return;
-  }
   std::vector<Group> groups(vu.size());
   for (size_t i = 0; i < vu.size(); ++i) {
     groups[i].key = vu[i];
     groups[i].vals = vg[i];
     groups[i].outs = og[i];
+  }
+  if (SkipsOnRescale()) {
+    SkipStep(groups);
+    PullImpl(okeys, outs, priority, true);
+    return;
   }
   raw_single_ = true;
   ReduceUpdate(groups, true);
@@ -1274,7 +1292,7 @@ bool KVStore::HostPipelined(std::vector<Group>& groups, bool write_outs) {
 // crosses the interconnect, and the consumer dequantises and sums.  Here every participating GPU is
 // a consumer: it reads all n code streams (peer loads), dequantises them into local scratch and
 // runs the ordinary fused reduce(+update) kernel on its own replica -- no root, no broadcast.
-void KVStore::ReduceUpdateCompressed(std::vector<Group>& groups, bool write_outs) {
+void KVStore::ReduceUpdateCompressed(std::vector<Group>& groups, bool write_outs, bool quantize_only) {
   Runtime* rt = Runtime::Get();
   ProcessGroup* pg = PG();
   const bool mp_mode = pg != nullptr;
@@ -1341,6 +1359,9 @@ void KVStore::ReduceUpdateCompressed(std::vector<Group>& groups, bool write_outs
       MXKV_CHECK(rc == 0) << "quantize launch failed: " << cudaGetErrorString(static_cast<cudaError_t>(rc));
       rt->launches++;
     }
+    // a skipped step (SkipStep): the residuals have advanced, nobody reads these codes (the next call's quantise
+    // is ordered after this call's on the same stream, and after every earlier call's reads by its end waits)
+    if (quantize_only) { StepKey(ks); continue; }
     // ---- 2. consumers: every GPU that holds (or must hold) a replica ----------------------------
     std::vector<int> consumers;
     if (mp_mode) consumers.push_back(pg->dev());
@@ -1361,12 +1382,17 @@ void KVStore::ReduceUpdateCompressed(std::vector<Group>& groups, bool write_outs
     const bool mp = fused && opt_.multi_precision;
     std::set<NDArray*> written;
     if (fused) StepKey(ks);
+    // every consumer's replica, master and state are made current before the first consumer updates its own: one
+    // made (or refreshed) afterwards would be copied from an updated replica and take the step twice
     for (int dev : consumers) {
       touch(dev);
       EnsureReplica(ks, dev);
       if (!stage_only && ks.local_world > 0) GatherLocal(ks);
       Replica& r = *FindReplica(ks, dev);
       if (fused) { if (ks.has_state) GatherState(ks); EnsureState(ks, r, mp); ks.state_world = 0; }
+    }
+    for (int dev : consumers) {
+      Replica& r = *FindReplica(ks, dev);
       DeviceGuard dg(dev);
       cudaStream_t s = rt->Dev(dev).stream;
       float* deq = nullptr;
@@ -2590,14 +2616,15 @@ void KVStore::UpdaterStep(bool str_keys, const std::vector<int>& ikeys, const st
     r->fresh = true;
     ks.local_world = 0;
     if (bind_only) continue;
-    if (SkipsOnRescale()) { StepKey(ks); continue; }
+    if (SkipsOnRescale() && grads[i].stype() == kRowSparseStorage) { StepKey(ks); continue; }
     if (grads[i].stype() == kRowSparseStorage) { sparse.emplace_back(key, grads[i]); continue; }
     Group grp;
     grp.key = key;
     grp.vals = {grads[i]};
     groups.push_back(grp);
   }
-  if (!groups.empty()) ReduceUpdate(groups, false);
+  if (!groups.empty() && SkipsOnRescale()) SkipStep(groups);
+  else if (!groups.empty()) ReduceUpdate(groups, false);
   for (auto& kg : sparse) PushRowSparse(GetKey(kg.first), {kg.second});
 }
 

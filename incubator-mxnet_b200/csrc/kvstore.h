@@ -249,7 +249,10 @@ class KVStore {
   void LaunchNormWorks(std::vector<NormClass>& classes, int opt_kind, const std::vector<int>& part_dev);
   void GatherLocal(KeyState& ks);
   bool HostPipelined(std::vector<Group>& groups, bool write_outs);
-  void ReduceUpdateCompressed(std::vector<Group>& groups, bool write_outs);
+  // quantize_only: quantise every pushed value (its residual advances) and count the update, nothing else
+  void ReduceUpdateCompressed(std::vector<Group>& groups, bool write_outs, bool quantize_only = false);
+  // a step that SkipsOnRescale: counted, weights and state untouched; under compression still quantised
+  void SkipStep(std::vector<Group>& groups);
   // the Python updater on (merged, root's stored value)
   void RunCallbackUpdater(KeyState& ks, Replica& root, const NDArray& merged);
   // rendezvous arguments (epoch left 0): the process group's ranks in `mode`, or one GPU alone (SYNC_NONE: the grid

@@ -327,9 +327,11 @@ def main():
 
     # 10. 2-bit gradient compression (tests/nightly/dist_sync_kvstore.py:330-426 in spirit): every worker quantises
     #     against its own residual, the dequantised values are what is summed -- inside the node from the codes,
-    #     between the nodes as float32 -- with and without an optimizer on the store, small and sharded keys
+    #     between the nodes as float32 -- with and without an optimizer on the store, small and sharded keys.  AdamW
+    #     skips its second step (rescale_grad inf): every rank still quantises, so the residuals advance
     thr = 0.5
-    for optname, kw in ((None, {}), ("sgd", dict(learning_rate=0.1, momentum=0.9))):
+    for optname, kw in ((None, {}), ("sgd", dict(learning_rate=0.1, momentum=0.9)),
+                        ("adamw", dict(learning_rate=0.01, wd=1e-2, epsilon=1e-6, rescale_grad=0.5))):
         kvc = mx.kv.create("dist_device_sync")
         kvc.set_gradient_compression({"type": "2bit", "threshold": thr})
         csizes = [3000, 300000]
@@ -338,10 +340,14 @@ def main():
         okv = O.OracleKVStore("device")
         okv.init(["c0", "c1"], [w.copy() for w in cw])
         if optname:
-            kvc.set_optimizer(mx.optimizer.create(optname, **kw))
-            okv.set_optimizer(O.OracleOptimizer(optname, **kw))
+            copt, oopt = mx.optimizer.create(optname, **kw), O.OracleOptimizer(optname, **kw)
+            kvc.set_optimizer(copt)
+            okv.set_optimizer(oopt)
         residual = [[np.zeros(e, np.float32) for _ in range(world)] for e in csizes]
-        for step in range(3):
+        for step in range(4 if optname == "adamw" else 3):
+            if optname == "adamw":
+                copt.rescale_grad = oopt.rescale_grad = float("inf") if step == 1 else 0.5
+                kvc.set_optimizer(copt)
             outs = [mx.nd.empty((e,), ctx) for e in csizes]
             kvc.pushpull(["c0", "c1"], [mx.nd.array(data(950 + 10 * step + j, (e,), rank), ctx)
                                         for j, e in enumerate(csizes)], out=outs)

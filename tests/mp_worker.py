@@ -300,6 +300,36 @@ def main():
                for r in range(world)]
         assert bits_equal(out.asnumpy(), O.sum_device(deq)), ("compression", step)
 
+    # 6b. 1-bit compression with a fused optimizer on a key of odd size (the scalar path): every rank reads the
+    #     others' codes between the two barriers and updates its own replica.  Then AdamW with a skipped second step
+    #     (rescale_grad inf): the ranks only quantise -- no barrier, no epoch -- and the steps after it continue from
+    #     the advanced residuals
+    E, thr = 10007, 0.0
+    for optname, kw in (("adam", dict(learning_rate=0.01, wd=1e-3)),
+                        ("adamw", dict(learning_rate=0.01, wd=1e-2, epsilon=1e-6, rescale_grad=0.5))):
+        kv6b = mx.kv.create("device")
+        kv6b.set_gradient_compression({"type": "1bit", "threshold": thr})
+        w0 = data(80, (E,), 0)
+        kv6b.init("c", mx.nd.array(w0, ctx))
+        opt6 = mx.optimizer.create(optname, **kw)
+        kv6b.set_optimizer(opt6)
+        oopt6 = O.OracleOptimizer(optname, **kw)
+        okv = O.OracleKVStore("device")
+        okv.init("c", w0.copy())
+        okv.set_optimizer(oopt6)
+        residual = [np.zeros(E, np.float32) for _ in range(world)]
+        for step in range(4):
+            if optname == "adamw":
+                opt6.rescale_grad = oopt6.rescale_grad = float("inf") if step == 1 else 0.5
+                kv6b.set_optimizer(opt6)
+            out = mx.nd.empty((E,), ctx)
+            kv6b.pushpull("c", mx.nd.array(data(81 + step, (E,), rank), ctx), out=out)
+            okv.push("c", [O.dequantize_1bit(O.quantize_1bit(data(81 + step, (E,), r), residual[r], thr), E, thr)
+                           for r in range(world)])
+            want = np.empty(E, np.float32)
+            okv.pull("c", want)
+            assert bits_equal(out.asnumpy(), want), ("compression", optname, step)
+
     # 7. NVLS: arrays bound to an NVSwitch multicast object -> multimem.ld_reduce / multimem.st kernel.
     #    The switch's summation order is not left-to-right: tolerance 1e-6 relative (the reference's
     #    own bound) against the oracle, and bit-identical replicas across ranks.

@@ -64,7 +64,8 @@ def test_single_gpu_paths(sim_lib):
     out = _run(sim_lib, 1, ["test_gpu_dense.py", "test_gpu_reference_kats.py", "test_gpu_rsp.py",
                             "test_gpu_norm_opt.py", "test_gpu_compression.py", "test_gpu_updater.py",
                             "test_gpu_y_trainer_nd.py", "test_gpu_y_semantics.py", "test_gpu_zz_threads.py",
-                            "test_gpu_lowp_optimizers.py", "test_gpu_rsp_edges.py", "test_gpu_norm_edges.py"])
+                            "test_gpu_lowp_optimizers.py", "test_gpu_rsp_edges.py", "test_gpu_norm_edges.py",
+                            "test_gpu_compression_edges.py"])
     assert _passed(out) >= 100, out[-500:]
 
 
@@ -77,7 +78,8 @@ def test_single_process_multi_gpu_paths(sim_lib, devices):
                                   "test_gpu_zzz_tree.py",
                                   "test_gpu_lowp_optimizers.py::test_multi_gpu_sharded_master_and_state_with_a_checkpoint",
                                   "test_gpu_rsp_edges.py::test_multi_gpu_localise_phase",
-                                  "test_gpu_norm_edges.py::test_sharded_key_with_small_chunks"],
+                                  "test_gpu_norm_edges.py::test_sharded_key_with_small_chunks",
+                                  "test_gpu_compression_edges.py::test_several_consumers_and_a_moving_slot"],
                extra=["-k", "not one_process_per_gpu"])
     assert _passed(out) >= 30, out[-500:]
 
